@@ -3,6 +3,7 @@
 // unicycle minimum-time OCP with the parameters of mpc_local_planner/cfg/test_mpc_optim_node.yaml, re-solved in a loop
 // through the mpc_local_planner::Controller mirror (include/mpcb200_controller.hpp) on top of the C ABI.
 #include <cstdio>
+#include <cstdlib>
 #include <vector>
 
 #include "../include/mpcb200_controller.hpp"
@@ -15,6 +16,8 @@ int main(int argc, char** argv)
     const bool adapt = argc > 2 && std::atoi(argv[2]) != 0;
     mpcb200_config cfg;
     mpcb200_default_config(&cfg);  // unicycle, N = 20, dt_ref = 0.3, minimum_time, xf fixed, point footprint, d_min 0.5
+    // solver/ipopt/max_cpu_time in seconds (default -1: no limit); a step stopped by it still succeeds (EarlyTerminated)
+    if (argc > 3) cfg.max_cpu_time = std::atof(argv[3]);
     cfg.k_max_obstacles_per_stage = 3;
     cfg.tol = 1e-8;
     std::vector<mpcb200::Obstacle> obstacles(3);

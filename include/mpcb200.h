@@ -21,7 +21,7 @@
 extern "C" {
 #endif
 
-#define MPCB200_VERSION 100
+#define MPCB200_VERSION 101
 
 /* ---- enums (ints in the struct so that ctypes/cgo bindings are trivial) -------------------------------- */
 
@@ -61,6 +61,8 @@ extern "C" {
 #define MPCB200_STATUS_MAX_ITER 1        /* iteration cap hit (reference: EarlyTerminated => step() still returns true) */
 #define MPCB200_STATUS_NUMERICAL_ERROR 2 /* inertia correction or line search failed */
 #define MPCB200_STATUS_INVALID_INPUT 3   /* NaN/inf in the instance's inputs */
+#define MPCB200_STATUS_MAX_TIME 4        /* time budget (max_cpu_time) exhausted; the current iterate is returned (reference: Ipopt
+                                            Maximum_CpuTime_Exceeded => EarlyTerminated => step() still returns true) */
 
 /* error codes */
 #define MPCB200_OK 0
@@ -157,6 +159,15 @@ typedef struct mpcb200_config {
        reference's 100 iterations (DESIGN.md "cold initial guess").  A locally convergent method inherits the homotopy class of
        its starting point, so the two modes may return different local optima of the same problem. */
     int reference_initial_guess;
+    /* solver/ipopt/max_cpu_time (src/controller.cpp:395-397; default -1 = no limit): a budget in seconds of DEVICE time per solve
+       call, counted from the start of the solve kernel (%globaltimer, one origin per launch shared by all its CTAs; copies, the
+       queue-order kernel and the costmap extraction are outside it).  An instance whose budget has run out when its next
+       iteration is evaluated stops with MPCB200_STATUS_MAX_TIME and returns its current iterate: exactly the outputs and warm
+       state of a solve with max_iter = the iterations it ran, only the status differs.  Instances the queue hands out after the
+       deadline get their initial guess (iters 0).  One budget per call: mpcb200_step_batch, _step_batch_costmap,
+       _solve_resident, _solve_stream (the whole queue); mpcb200_step_batch_multi applies it per device.  <= 0 or +inf: no
+       budget; NaN: E_INVALID.  Not with MPCB200_OPT_SOLVE_MODE 1 (the solve returns E_UNSUPPORTED). */
+    double max_cpu_time;
 } mpcb200_config;
 
 /* Per-instance obstacle lists, fixed stride: instance b owns obstacles [b*max_per_instance, b*max_per_instance+count[b]).

@@ -243,8 +243,10 @@ class Controller
         }
         else
         {
-            // success iff the solver status is Converged or EarlyTerminated (SURVEY App. B.1)
-            _ocp_successful = (status == MPCB200_STATUS_CONVERGED || status == MPCB200_STATUS_MAX_ITER);
+            // success iff the solver status is Converged or EarlyTerminated (SURVEY App. B.1).  EarlyTerminated covers the iteration
+            // cap and the time budget (max_cpu_time): [EXT] Ipopt's Maximum_CpuTime_Exceeded is taken to map to EarlyTerminated like
+            // Maximum_Iterations_Exceeded -- the mapping lives in corbo's Ipopt wrapper, which is not part of the reference tree.
+            _ocp_successful = (status == MPCB200_STATUS_CONVERGED || status == MPCB200_STATUS_MAX_ITER || status == MPCB200_STATUS_MAX_TIME);
             // a failed solve (numerical error, invalid input) leaves no trajectory to warm-start from: the device keeps the
             // instance cold, and the grid counts as empty here (the reference's planner resets the controller after a failed step)
             _grid_empty = !_ocp_successful;

@@ -25,7 +25,7 @@ COST_LEFT_SUM, COST_TRAPEZOIDAL = 0, 1
 OBJ_MINIMUM_TIME, OBJ_QUADRATIC_FORM, OBJ_MINIMUM_TIME_VIA_POINTS = 0, 1, 2
 FOOTPRINT_POINT, FOOTPRINT_CIRCULAR, FOOTPRINT_TWO_CIRCLES, FOOTPRINT_LINE, FOOTPRINT_POLYGON = 0, 1, 2, 3, 4
 OBST_POINT, OBST_CIRCLE, OBST_LINE = 0, 1, 2
-STATUS_CONVERGED, STATUS_MAX_ITER, STATUS_NUMERICAL_ERROR, STATUS_INVALID_INPUT = 0, 1, 2, 3
+STATUS_CONVERGED, STATUS_MAX_ITER, STATUS_NUMERICAL_ERROR, STATUS_INVALID_INPUT, STATUS_MAX_TIME = 0, 1, 2, 3, 4
 E_INVALID, E_UNSUPPORTED, E_CUDA, E_NOMEM, E_NODEVICE = -1, -2, -3, -4, -5
 F_X, F_U, F_NU, F_S, F_LAM, F_KKT, F_STEP, F_SCAL, F_OBSIDX, F_OBSGIDX = range(10)
 PHASE_INIT, PHASE_ASSOCIATE, PHASE_EVAL, PHASE_KKT, PHASE_LINESEARCH = range(5)
@@ -89,6 +89,7 @@ class Config(C.Structure):
         ("cost_integration", C.c_int),
         ("hybrid_cost_minimum_time", C.c_int),
         ("reference_initial_guess", C.c_int),
+        ("max_cpu_time", C.c_double),
     ]
 
     def copy(self):
@@ -154,6 +155,7 @@ def default_config():
     c.terminal_ball_gamma = 5.0
     c.cost_integration = COST_LEFT_SUM
     c.hybrid_cost_minimum_time = 0
+    c.max_cpu_time = -1.0
     return c
 
 

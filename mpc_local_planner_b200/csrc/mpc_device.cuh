@@ -432,6 +432,17 @@ __device__ __forceinline__ void dev_associate(const Cfg& c, const WsLayout& L, d
     __syncwarp();
 }
 
+// ---- time budget of a solve (mpcb200_config.max_cpu_time) ----
+// %globaltimer: nanoseconds of one clock for the whole device (clock64 counts cycles of one SM, at whatever clock it runs).
+#define NO_DEADLINE 0xFFFFFFFFFFFFFFFFull
+__device__ __forceinline__ unsigned long long global_ns()
+{
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+__device__ __forceinline__ bool budget_expired(unsigned long long deadline) { return deadline != NO_DEADLINE && global_ns() >= deadline; }
+
 // ---- shared scratch of the CTA-wide phases ----
 struct CtaShared
 {
@@ -441,6 +452,7 @@ struct CtaShared
     int hist[CLIP_BINS + 1];
     double mu, alpha, a_dual;
     int fin, accept;
+    unsigned long long deadline;   // %globaltimer value at which the solve's time budget runs out (NO_DEADLINE: none)
 };
 
 __device__ __forceinline__ double shfl_xor_d(double v, int o) { return __shfl_xor_sync(FULLMASK, v, o); }
@@ -460,7 +472,8 @@ __device__ __forceinline__ void evalacc_warp_reduce(EvalAcc& a)
 }
 
 // ---- PHASE_EVAL (whole CTA, lane per stage): stage functions + derivatives -> condensed KKT records, KKT error,
-//      convergence test and barrier update.  Returns 1 (uniform) when the instance terminates. ----
+//      convergence test (and the time budget: thread 0 reads the clock, sh.fin broadcasts its decision) and barrier update.
+//      Returns 1 (uniform) when the instance terminates. ----
 template <bool LINES>
 __device__ __forceinline__ int dev_eval(const Cfg& c, const WsLayout& L, double* W, double uprev_dt, CtaShared& sh, int tid, int nt)
 {
@@ -476,7 +489,7 @@ __device__ __forceinline__ int dev_eval(const Cfg& c, const WsLayout& L, double*
     {
         for (int w = 1; w < nw; ++w) evalacc_merge(a, sh.eacc[w]);
         int fin = 0;
-        sh.mu = eval_finish(c, L, W, a, true, &fin);
+        sh.mu = eval_finish(c, L, W, a, true, &fin, budget_expired(sh.deadline));
         sh.fin = fin;
     }
     __syncthreads();

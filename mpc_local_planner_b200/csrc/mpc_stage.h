@@ -480,7 +480,9 @@ HD inline void eval_stage(const Cfg& c, const WsLayout& L, double* W, double* G,
 
 // After the warp reduction: convergence test, monotone barrier update (Ipopt's Fiacco-McCormick rule), scalars.
 // Returns the barrier parameter to finalise the gradients with; *finished is set when the instance terminates.
-HD inline double eval_finish(const Cfg& c, const WsLayout& L, double* W, const EvalAcc& a, bool write, int* finished)
+// expired: the time budget of the solve (max_cpu_time) has run out.  It is tested after the iteration cap, so an instance stopped
+// here at iteration j holds exactly what a solve with max_iter = j leaves; only the status differs.
+HD inline double eval_finish(const Cfg& c, const WsLayout& L, double* W, const EvalAcc& a, bool write, int* finished, bool expired = false)
 {
     double mu = ASC(MPCB200_SC_MU);
     const double tol = c.tol, mu_min = tol / 10.0;
@@ -493,6 +495,7 @@ HD inline double eval_finish(const Cfg& c, const WsLayout& L, double* W, const E
     int fin = 0, status = -1;
     if (e0 <= tol) { fin = 1; status = MPCB200_STATUS_CONVERGED; }
     else if (iter >= c.max_iter) { fin = 1; status = MPCB200_STATUS_MAX_ITER; }
+    else if (expired) { fin = 1; status = MPCB200_STATUS_MAX_TIME; }
     if (!(e0 == e0)) { fin = 1; status = MPCB200_STATUS_NUMERICAL_ERROR; }
     if (!fin)
     {

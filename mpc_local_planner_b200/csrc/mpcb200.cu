@@ -97,7 +97,11 @@ __global__ void __launch_bounds__(MAX_GROUP_WARPS * 32, 3) phase_kernel(const __
     if (phase >= MPCB200_PHASE_EVAL && Gp[L.oSCAL + MPCB200_SC_STATUS] >= 0.0) return;  // finished instance: exact no-op (uniform over the CTA)
     double* W = reinterpret_cast<double*>(dyn_smem + IMG_HEAD);
     const uint32_t bar = smem_addr(dyn_smem);
-    if (tid == 0) { mbar_init(bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+    if (tid == 0)
+    {
+        mbar_init(bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        sh.deadline = NO_DEADLINE;   // one phase for every instance: no solve, no clock of a solve (max_cpu_time: fused kernel only)
+    }
     __syncthreads();
     stage_in(W, Gp, img_words, bar, 0, tid);
     switch (phase)
@@ -183,6 +187,8 @@ struct FusedArgs
     unsigned long long* counters;
     unsigned long long* sm_sync;   // [SMs] phase alignment words (nullptr: off)
     int sm_gates;                  // 3: gates before eval, KKT and line search; 2: before KKT and line search only
+    unsigned long long budget_ns;  // time budget of the launch (max_cpu_time), 0: none
+    unsigned long long* origin;    // %globaltimer at the start of the launch: the first CTA sets it (zeroed before the launch)
 };
 // ---- phase alignment of the CTAs that share an SM ---------------------------------------------------------------------------
 // The solve kernel's iteration is ~128 KB of straight fp64 code, several times an SM's instruction cache: CTAs that sit on the
@@ -236,14 +242,22 @@ __device__ __forceinline__ void sms_arrive(unsigned long long* st, unsigned phas
 // up (2-3 ms into the step) ends 2-3 ms later than if it had been among the first.  Nothing predicts the iteration count of a cold
 // instance from its geometry (correlations < 0.2 on the BASELINE instances), but a robot that was hard in the last cycle tends to be
 // hard in this one, so the history is the hint.  Counting sort (descending, stable) by min(iters, 1023) in one CTA.
-__global__ void __launch_bounds__(1024) order_by_history_kernel(const int* __restrict__ prev_iters, int B, int* __restrict__ order)
+// An instance the time budget stopped (MPCB200_STATUS_MAX_TIME) counts as needing max_iter iterations whatever it ran: otherwise
+// the instances the queue never reached (iters 0) would go last again and stay unsolved in every cycle.
+__device__ __forceinline__ int history_key(const int* prev_iters, const int* prev_status, int max_iter, int i)
+{
+    const int k = prev_status[i] == MPCB200_STATUS_MAX_TIME ? max_iter : prev_iters[i];
+    return k < 0 ? 0 : (k > 1023 ? 1023 : k);
+}
+__global__ void __launch_bounds__(1024) order_by_history_kernel(const int* __restrict__ prev_iters, const int* __restrict__ prev_status, int max_iter,
+                                                                int B, int* __restrict__ order)
 {
     __shared__ int hist[1024];
     __shared__ int warp_tot[32];
     const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
     hist[t] = 0;
     __syncthreads();
-    for (int i = t; i < B; i += 1024) { int k = prev_iters[i]; k = k < 0 ? 0 : (k > 1023 ? 1023 : k); atomicAdd(&hist[1023 - k], 1); }
+    for (int i = t; i < B; i += 1024) atomicAdd(&hist[1023 - history_key(prev_iters, prev_status, max_iter, i)], 1);
     __syncthreads();
     // exclusive scan of hist (bucket 0 = the longest)
     const int v = hist[t];
@@ -263,10 +277,7 @@ __global__ void __launch_bounds__(1024) order_by_history_kernel(const int* __res
         int pos = hist[t];
         const int key = 1023 - t;
         for (int i = 0; i < B; ++i)
-        {
-            int k = prev_iters[i]; k = k < 0 ? 0 : (k > 1023 ? 1023 : k);
-            if (k == key) order[pos++] = i;
-        }
+            if (history_key(prev_iters, prev_status, max_iter, i) == key) order[pos++] = i;
     }
 }
 
@@ -280,7 +291,19 @@ __global__ void __launch_bounds__(MAX_GROUP_WARPS * 32, 3) solve_fused_kernel(co
     const int N = L.N;
     double* W = reinterpret_cast<double*>(dyn_smem + IMG_HEAD);
     const uint32_t bar = smem_addr(dyn_smem);
-    if (tid == 0) { mbar_init(bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+    if (tid == 0)
+    {
+        mbar_init(bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        // the time budget: one origin for the whole launch, the %globaltimer reading of the CTA that starts first
+        unsigned long long deadline = NO_DEADLINE;
+        if (a.budget_ns)
+        {
+            const unsigned long long now = global_ns(), prev = atomicCAS(a.origin, 0ull, now), t0 = prev ? prev : now;
+            deadline = t0 + a.budget_ns;
+            if (deadline < t0 || deadline == NO_DEADLINE) deadline = NO_DEADLINE - 1;   // saturate
+        }
+        sh.deadline = deadline;
+    }
     CudaWarp<EXT> ex;
     ex.lane = lane;
     if (wid == 0) kkt_warp_setup<EXT>(ex, c.variable_dt);
@@ -355,6 +378,7 @@ __global__ void __launch_bounds__(MAX_GROUP_WARPS * 32, 3) solve_fused_kernel(co
                 }
 #undef PHASE_GATE
                 if (sms) { if (tid == 0) sms_leave(sms); __syncthreads(); }
+                if (ASC(MPCB200_SC_STATUS) == (double)MPCB200_STATUS_MAX_TIME) break;   // the budget spans the outer iterations
             }
             // a failed solve leaves nothing to warm-start from
             if (tid == 0 && ASC(MPCB200_SC_STATUS) == (double)MPCB200_STATUS_NUMERICAL_ERROR) ASC(MPCB200_SC_COLD) = 1.0;
@@ -467,7 +491,9 @@ struct mpcb200_handle
     int fused_grid;  // CTAs of the last fused launch
     int order_by_history; // MPCB200_OPT_ORDER_BY_HISTORY: batch queue longest-first by the previous solve's iteration counts
     int hist_B;           // batch size of the last batch solve whose iteration counts are in d_iters (0: none)
-    int *d_prev_iters, *d_order;
+    int *d_prev_iters, *d_prev_status, *d_order;
+    unsigned long long budget_ns;   // max_cpu_time in ns (0: no budget)
+    unsigned long long* d_origin;   // start of the current solve launch (%globaltimer), see FusedArgs
     int sm_phase_sync;    // MPCB200_OPT_SM_PHASE_SYNC: co-resident CTAs of the solve kernel enter the phases together
     unsigned long long* d_smsync;
     int max_ctas_per_sm;  // MPCB200_OPT_CTAS_PER_SM: cap on the resident CTAs per SM of the solve kernel (0 = what fits)
@@ -514,6 +540,7 @@ extern "C" void mpcb200_default_config(mpcb200_config* c)
     for (int i = 0; i < 9; ++i) c->terminal_ball_S[i] = (i % 4 == 0) ? 1.0 : 0.0;
     c->cost_integration = MPCB200_COST_LEFT_SUM;
     c->hybrid_cost_minimum_time = 0;
+    c->max_cpu_time = -1.0;
 }
 
 
@@ -537,6 +564,7 @@ static int validate_config(const mpcb200_config* c, std::string& why)
     if (c->variable_dt && !(c->dt_ub > c->dt_lb)) { why = "dt_ub must exceed dt_lb"; return MPCB200_E_INVALID; }
     if (has_mintime(*c) && !c->variable_dt) { why = "minimum_time objectives need variable_dt"; return MPCB200_E_INVALID; }
     if (!(c->tol > 0) || c->max_iter < 1) { why = "tol > 0 and max_iter >= 1 required"; return MPCB200_E_INVALID; }
+    if (c->max_cpu_time != c->max_cpu_time) { why = "max_cpu_time is NaN (a budget in seconds; <= 0 or +inf: none)"; return MPCB200_E_INVALID; }
     for (int i = 0; i < 2; ++i)
         if (!(c->u_ub[i] > c->u_lb[i])) { why = "u_ub must exceed u_lb"; return MPCB200_E_INVALID; }
     // one CTA keeps the instance's resident prefix in shared memory: that bounds the horizon (about (56 + 6 RS + 4 K) N words)
@@ -572,7 +600,10 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
     make_layout(cfg, MAX_OBST, MAX_VP, h->L);
     h->n_cap = cfg->n; h->d_resample = nullptr; h->d_cm = nullptr; h->cm_cap = 0; h->costmap_ms = 0.0; h->d_fz = nullptr; h->fz_cap = 0;
     h->uprev_dt = 0.0; h->has_obst = h->has_vp = h->has_xinit = h->has_reinit = 0; h->obst_max = h->vp_max = 0; h->has_lines = 0;
-    h->solve_mode = 0; h->timing_mask = 1u << MPCB200_PHASE_KKT; h->fused_grid = 0; h->max_ctas_per_sm = 0; h->sm_phase_sync = -1; h->d_smsync = nullptr; h->order_by_history = 1; h->hist_B = 0; h->d_prev_iters = h->d_order = nullptr;
+    h->solve_mode = 0; h->timing_mask = 1u << MPCB200_PHASE_KKT; h->fused_grid = 0; h->max_ctas_per_sm = 0; h->sm_phase_sync = -1; h->d_smsync = nullptr; h->order_by_history = 1; h->hist_B = 0; h->d_prev_iters = h->d_prev_status = h->d_order = nullptr;
+    h->d_origin = nullptr;
+    // seconds -> ns, rounded up; a budget beyond 2^62 ns (146 years) is no budget
+    h->budget_ns = (cfg->max_cpu_time > 0.0 && cfg->max_cpu_time * 1e9 < 4611686018427387904.0) ? (unsigned long long)ceil(cfg->max_cpu_time * 1e9) : 0ull;
 #define CKC(call)                                                                                                  \
     do {                                                                                                           \
         cudaError_t e_ = (call);                                                                                   \
@@ -594,7 +625,8 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
     CKC(cudaMalloc(&h->d_xinit, B * N * 3 * 8)); CKC(cudaMalloc(&h->d_reinit, B));
     CKC(cudaMalloc(&h->d_useq, B * N * 2 * 8)); CKC(cudaMalloc(&h->d_xseq, B * N * 3 * 8)); CKC(cudaMalloc(&h->d_dt, B * 8));
     CKC(cudaMalloc(&h->d_kkt, B * 8)); CKC(cudaMalloc(&h->d_upacked, B * (N - 1) * 2 * 8));
-    CKC(cudaMalloc(&h->d_status, B * 4)); CKC(cudaMalloc(&h->d_iters, B * 4)); CKC(cudaMalloc(&h->d_nactive, 8)); CKC(cudaMalloc(&h->d_queue, 4)); CKC(cudaMalloc(&h->d_smsync, 1024 * 8)); CKC(cudaMalloc(&h->d_prev_iters, B * 4)); CKC(cudaMalloc(&h->d_order, B * 4));
+    CKC(cudaMalloc(&h->d_status, B * 4)); CKC(cudaMalloc(&h->d_iters, B * 4)); CKC(cudaMalloc(&h->d_nactive, 8)); CKC(cudaMalloc(&h->d_queue, 4)); CKC(cudaMalloc(&h->d_smsync, 1024 * 8)); CKC(cudaMalloc(&h->d_prev_iters, B * 4)); CKC(cudaMalloc(&h->d_prev_status, B * 4)); CKC(cudaMalloc(&h->d_order, B * 4));
+    CKC(cudaMalloc(&h->d_origin, 8));
     CKC(cudaMalloc(&h->d_counters, CNT_WORDS * 8)); CKC(cudaMemsetAsync(h->d_counters, 0, CNT_WORDS * 8, h->stream));
     CKC(allow_smem(phase_kernel<false>)); CKC(allow_smem(phase_kernel<true>));
     CKC(allow_smem(kkt_warp_kernel<false>)); CKC(allow_smem(kkt_warp_kernel<true>));
@@ -627,7 +659,7 @@ extern "C" void mpcb200_destroy(mpcb200_handle* h)
     cudaSetDevice(h->device);
     cudaStreamSynchronize(h->stream);
     void* ptrs[] = {h->ws, h->d_x0, h->d_xf, h->d_uprev, h->d_obst, h->d_obst_count, h->d_obst_type, h->d_vp, h->d_vp_count, h->d_xinit,
-                    h->d_reinit, h->d_useq, h->d_xseq, h->d_dt, h->d_kkt, h->d_upacked, h->d_status, h->d_iters, h->d_nactive, h->d_queue, h->d_flush, h->d_counters, h->d_smsync, h->d_prev_iters, h->d_order};
+                    h->d_reinit, h->d_useq, h->d_xseq, h->d_dt, h->d_kkt, h->d_upacked, h->d_status, h->d_iters, h->d_nactive, h->d_queue, h->d_flush, h->d_counters, h->d_smsync, h->d_prev_iters, h->d_prev_status, h->d_order, h->d_origin};
     for (void* p : ptrs) if (p) cudaFree(p);
     void* sptrs[] = {h->s_x0, h->s_xf, h->s_uprev, h->s_obst, h->s_vp, h->s_useq, h->s_xseq, h->s_dt, h->s_kkt, h->s_upacked, h->s_obst_count,
                      h->s_obst_type, h->s_vp_count, h->s_status, h->s_iters, h->d_resample, h->d_cm, h->d_fz};
@@ -830,11 +862,14 @@ static int launch_fused(mpcb200_handle* h, int total, int queue_mode, int force_
     a.img_words = image_words(h); a.queue = h->d_queue; a.counters = h->d_counters;
     a.sm_sync = nullptr; a.sm_gates = h->sm_phase_sync == 2 ? 2 : 3;
     a.order = nullptr;
+    a.budget_ns = h->budget_ns; a.origin = h->d_origin;
+    if (h->budget_ns) CK(cudaMemsetAsync(h->d_origin, 0, 8, h->stream));
     if (!queue_mode && h->order_by_history && h->hist_B == total && total > h->num_sms)
     {
-        // (d_iters is rewritten by this solve: order from a copy)
+        // (d_iters and d_status are rewritten by this solve: order from copies)
         CK(cudaMemcpyAsync(h->d_prev_iters, h->d_iters, (size_t)total * 4, cudaMemcpyDeviceToDevice, h->stream));
-        order_by_history_kernel<<<1, 1024, 0, h->stream>>>(h->d_prev_iters, total, h->d_order);
+        CK(cudaMemcpyAsync(h->d_prev_status, h->d_status, (size_t)total * 4, cudaMemcpyDeviceToDevice, h->stream));
+        order_by_history_kernel<<<1, 1024, 0, h->stream>>>(h->d_prev_iters, h->d_prev_status, h->cfg.max_iter, total, h->d_order);
         h->stats.launches_total += 1;
         a.order = h->d_order;
     }
@@ -925,6 +960,15 @@ static int collect_fused_counters(mpcb200_handle* h)
     h->stats.kkt_sweeps += (long long)cnt[CNT_KKT_SWEEPS];
     h->stats.launches[MPCB200_PHASE_KKT] += (long long)cnt[CNT_KKT_INST];
     CK(cudaMemsetAsync(h->d_counters, 0, sizeof(cnt), h->stream));
+    return 0;
+}
+
+// the phased mode queues the iterations from the host: its launches do not share the solve kernel's clock
+static int check_budget_mode(mpcb200_handle* h)
+{
+    if (h->budget_ns && h->solve_mode == 1)
+        return set_err(h, MPCB200_E_UNSUPPORTED, "max_cpu_time (a time budget) needs the fused solve kernel: MPCB200_OPT_SOLVE_MODE 1 "
+                                                 "(one launch per phase) has no budget; set the option to 0 or max_cpu_time to -1");
     return 0;
 }
 
@@ -1021,6 +1065,7 @@ extern "C" int mpcb200_step_batch(mpcb200_handle* h, int B, const double* x0, co
 {
     int rc = check_batch(h, B);
     if (rc) return rc;
+    if ((rc = check_budget_mode(h))) return rc;
     CK(cudaSetDevice(h->device));
     if (h->solve_mode == 1)
     {
@@ -1052,6 +1097,7 @@ extern "C" int mpcb200_upload_inputs(mpcb200_handle* h, int B, const double* x0,
 extern "C" int mpcb200_solve_resident(mpcb200_handle* h, int cold, double* solve_time_s)
 {
     if (!h || h->B < 1) return set_err(h, MPCB200_E_INVALID, "no resident inputs: call mpcb200_upload_inputs first");
+    if (int rc = check_budget_mode(h)) return rc;
     CK(cudaSetDevice(h->device));
     return solve_device(h, h->B, cold ? 1 : 0, solve_time_s);
 }
@@ -1382,6 +1428,7 @@ extern "C" int mpcb200_step_batch_costmap(mpcb200_handle* h, int B, const double
     int rc = check_batch(h, B);
     if (rc) return rc;
     if (max_per_instance < 1 || max_per_instance > MAX_OBST_LIST) return set_err(h, MPCB200_E_UNSUPPORTED, "step_batch_costmap: 1..2048 obstacles per instance");
+    if ((rc = check_budget_mode(h))) return rc;
     CK(cudaSetDevice(h->device));
     // room for the lists in the batch's obstacle arrays
     if ((rc = reserve_obstacles(h, false, (size_t)h->max_batch, max_per_instance))) return rc;
