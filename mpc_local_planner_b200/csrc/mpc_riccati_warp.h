@@ -195,9 +195,10 @@ template <bool EXT>
 HD inline void rw_column(int var, int dt_free, int* fo, double* fc, int* own)
 {
     // column `var` of FF_k: x+ = x + a x_2 + B v + e th^0 + d th^1,  p+ = v,  th^ = th^
-    for (int a = 0; a < 3; ++a) { fo[a] = REC_ZERO; fc[a] = 0.0; }
+    // (no runtime index into fo / fc: the lane programs live in the warp's lane state, which must stay in registers)
+    for (int a = 0; a < 3; ++a) { fo[a] = REC_ZERO; fc[a] = (var < 2 && a == var) ? 1.0 : 0.0; }
     *own = -1;
-    if (var < 2) fc[var] = 1.0;
+    if (var < 2) {}
     else if (var == 2) { for (int a = 0; a < 3; ++a) fo[a] = MPCB200_K_A + a; fc[2] = 1.0; }
     else if (var < 5) {}
     else if (var < 7) { for (int a = 0; a < 3; ++a) fo[a] = MPCB200_K_B + 2 * a + (var - 5); *own = 3 + (var - 5); }
@@ -420,19 +421,42 @@ HD inline void rw_stage_map(const double* rec, const double* mm, int dt_free, do
     q.M[3][3] = -g[6]; q.M[3][4] = -g[7]; q.M[4][3] = -g[8]; q.M[4][4] = -g[9];
     q.b[3] = -g[10]; q.b[4] = -g[11];
 }
-// a <- a o b  (first b, then a):  M = Ma Mb,  b = Ma bb + ba
+// Composition a o b (first b, then a):  M = Ma Mb,  b = Ma bb + ba.  Two in-place forms, so that no third map is live: the
+// scan operands stay in registers.  Both form every entry by the same expression.
+HD inline double rw_dot5(const double* r, double c0, double c1, double c2, double c3, double c4)
+{
+    return ((r[0] * c0 + r[1] * c1) + (r[2] * c2 + r[3] * c3)) + r[4] * c4;
+}
+// a <- a o b, row by row (row i of the result needs row i of a only)
 HD inline void rw_compose(RwMap& a, const RwMap& b)
 {
-    RwMap r;
 #pragma unroll
     for (int i = 0; i < 5; ++i)
     {
+        double r[5];
 #pragma unroll
-        for (int j = 0; j < 5; ++j)
-            r.M[i][j] = ((a.M[i][0] * b.M[0][j] + a.M[i][1] * b.M[1][j]) + (a.M[i][2] * b.M[2][j] + a.M[i][3] * b.M[3][j])) + a.M[i][4] * b.M[4][j];
-        r.b[i] = (((a.M[i][0] * b.b[0] + a.M[i][1] * b.b[1]) + (a.M[i][2] * b.b[2] + a.M[i][3] * b.b[3])) + a.M[i][4] * b.b[4]) + a.b[i];
+        for (int j = 0; j < 5; ++j) r[j] = rw_dot5(a.M[i], b.M[0][j], b.M[1][j], b.M[2][j], b.M[3][j], b.M[4][j]);
+        a.b[i] = rw_dot5(a.M[i], b.b[0], b.b[1], b.b[2], b.b[3], b.b[4]) + a.b[i];
+#pragma unroll
+        for (int j = 0; j < 5; ++j) a.M[i][j] = r[j];
     }
-    a = r;
+}
+// b <- a o b, column by column (column j of the result needs column j of b only)
+HD inline void rw_compose_onto(const RwMap& a, RwMap& b)
+{
+    double r[5];
+#pragma unroll
+    for (int i = 0; i < 5; ++i) r[i] = rw_dot5(a.M[i], b.b[0], b.b[1], b.b[2], b.b[3], b.b[4]) + a.b[i];
+#pragma unroll
+    for (int i = 0; i < 5; ++i) b.b[i] = r[i];
+#pragma unroll
+    for (int j = 0; j < 5; ++j)
+    {
+#pragma unroll
+        for (int i = 0; i < 5; ++i) r[i] = rw_dot5(a.M[i], b.M[0][j], b.M[1][j], b.M[2][j], b.M[3][j], b.M[4][j]);
+#pragma unroll
+        for (int i = 0; i < 5; ++i) b.M[i][j] = r[i];
+    }
 }
 // replay the stages [k0, k1) from the state y at stage k0: dw_k -> stp; returns the state at k1 in y
 template <bool EXT>
@@ -606,8 +630,7 @@ HD inline int kkt_warp_attempt(Exec& ex, const Cfg& c, int N, double* recs, doub
         {
             RwMap q;
             rw_stage_map<EXT>(recs + (size_t)k * RSTR, mms + (size_t)k * T::MSTR, dt_free, th[1], q);
-            rw_compose(q, ls.out);
-            ls.out = q;
+            rw_compose_onto(q, ls.out);
         }
     });
     for (int d = 1; d < 32; d <<= 1)

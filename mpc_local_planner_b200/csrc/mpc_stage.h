@@ -664,19 +664,25 @@ HD inline void ls_stage_steps(const Cfg& c, const WsLayout& L, double* W, double
     acc.dJ += dJ;
     // curvature dz' H dz of this stage's block (+ cross block with stage k-1, + border)
     {
+        // (unrolled over the largest block with the bound as a condition: st stays in registers)
         const int nv = (k <= N - 2) ? 5 : 3;
-        double st[5] = {dx[0], dx[1], dx[2], du[0], du[1]};
+        const double st[5] = {dx[0], dx[1], dx[2], du[0], du[1]};
         double cv = 0.0;
-        for (int i = 0; i < nv; ++i)
-            for (int j = 0; j < nv; ++j)
+#pragma unroll
+        for (int i = 0; i < 5; ++i)
+#pragma unroll
+            for (int j = 0; j < 5; ++j)
             {
+                if (i >= nv || j >= nv) continue;
                 const int a = i < j ? i : j, b = i < j ? j : i;
                 cv += st[i] * (AKKT(MPCB200_K_H + hidx(a, b), k) + (a == b ? delta : 0.0)) * st[j];
             }
         if (k >= 1 && k <= N - 2)
             for (int i = 0; i < 2; ++i) cv += 2.0 * ASTEP(3 + i, k - 1) * AKKT(MPCB200_K_C + i, k) * du[i];
         if (c.variable_dt)  // border (the terminal record carries one only with the trapezoidal rule)
-            for (int i = 0; i < nv; ++i) cv += 2.0 * ddt * AKKT(MPCB200_K_HB + i, k) * st[i];
+#pragma unroll
+            for (int i = 0; i < 5; ++i)
+                if (i < nv) cv += 2.0 * ddt * AKKT(MPCB200_K_HB + i, k) * st[i];
         if (c.variable_dt && k == N - 1) cv += ddt * ddt * (ASC(MPCB200_SC_HTT) + delta);
         acc.curv += cv;
     }

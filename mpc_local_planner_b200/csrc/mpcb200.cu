@@ -281,8 +281,18 @@ __global__ void __launch_bounds__(1024) order_by_history_kernel(const int* __res
     }
 }
 
-template <bool LINES, bool EXT>
-__global__ void __launch_bounds__(MAX_GROUP_WARPS * 32, 3) solve_fused_kernel(const __grid_constant__ Cfg c, const __grid_constant__ WsLayout L, const __grid_constant__ FusedArgs a)
+// CTA shapes of the solve kernel.  The launch bound sets the register budget of a thread (255 in both shapes), so it follows
+// the shape a launch uses: horizons up to 64 grid points run 1-2 warps, and their shared-memory image (about 55 KB at N = 50)
+// lets 4 CTAs share an SM; longer horizons run 3-4 warps with an image of about 70 KB and more (90 KB at N = 80), so
+// shared memory allows 2 CTAs per SM from N = 80 on, and the bound keeps them at 2 below that.  A budget set for a shape a
+// launch does not use spills the iteration's operands to local memory.
+#define SMALL_GROUP_WARPS 2
+template <int WARPS> struct FusedShape;
+template <> struct FusedShape<SMALL_GROUP_WARPS> { static constexpr int MIN_CTAS = 4; };
+template <> struct FusedShape<MAX_GROUP_WARPS> { static constexpr int MIN_CTAS = 2; };
+
+template <bool LINES, bool EXT, int WARPS>
+__global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve_fused_kernel(const __grid_constant__ Cfg c, const __grid_constant__ WsLayout L, const __grid_constant__ FusedArgs a)
 {
     extern __shared__ __align__(128) unsigned char dyn_smem[];
     __shared__ CtaShared sh;
@@ -630,8 +640,12 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
     CKC(cudaMalloc(&h->d_counters, CNT_WORDS * 8)); CKC(cudaMemsetAsync(h->d_counters, 0, CNT_WORDS * 8, h->stream));
     CKC(allow_smem(phase_kernel<false>)); CKC(allow_smem(phase_kernel<true>));
     CKC(allow_smem(kkt_warp_kernel<false>)); CKC(allow_smem(kkt_warp_kernel<true>));
-    CKC(allow_smem(solve_fused_kernel<false, false>)); CKC(allow_smem(solve_fused_kernel<false, true>));
-    CKC(allow_smem(solve_fused_kernel<true, false>)); CKC(allow_smem(solve_fused_kernel<true, true>));
+#define ALLOW_FUSED(W_)                                                                                              \
+    CKC(allow_smem(solve_fused_kernel<false, false, W_>)); CKC(allow_smem(solve_fused_kernel<false, true, W_>));     \
+    CKC(allow_smem(solve_fused_kernel<true, false, W_>)); CKC(allow_smem(solve_fused_kernel<true, true, W_>))
+    ALLOW_FUSED(SMALL_GROUP_WARPS);
+    ALLOW_FUSED(MAX_GROUP_WARPS);
+#undef ALLOW_FUSED
     CKC(cudaMallocHost(&h->h_nactive, 8));
     h->stream_cap = 0;
     h->s_x0 = h->s_xf = h->s_uprev = h->s_obst = h->s_vp = h->s_useq = h->s_xseq = h->s_dt = h->s_kkt = h->s_upacked = nullptr;
@@ -877,11 +891,12 @@ static int launch_fused(mpcb200_handle* h, int total, int queue_mode, int force_
     const size_t smem = IMG_HEAD + (size_t)a.img_words * 8;
     if (smem > MAX_IMG_SMEM) return set_err(h, MPCB200_E_UNSUPPORTED, "the instance does not fit in shared memory");
     const int threads = group_threads(h);
-    const bool ext = kkt_is_ext(h->cfg);
+    const bool ext = kkt_is_ext(h->cfg), small = threads <= SMALL_GROUP_WARPS * 32;
     int per_sm = 0;
-#define FUSED_DO(LN, EX)                                                                                                       \
+#define FUSED_DO(LN, EX) do { if (small) FUSED_SHAPE(LN, EX, SMALL_GROUP_WARPS); else FUSED_SHAPE(LN, EX, MAX_GROUP_WARPS); } while (0)
+#define FUSED_SHAPE(LN, EX, WS)                                                                                                \
     do {                                                                                                                       \
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, solve_fused_kernel<LN, EX>, threads, smem));                 \
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, solve_fused_kernel<LN, EX, WS>, threads, smem));             \
         if (per_sm < 1) return set_err(h, MPCB200_E_UNSUPPORTED, "the solve kernel does not fit on an SM with this configuration"); \
         if (h->max_ctas_per_sm > 0 && per_sm > h->max_ctas_per_sm) per_sm = h->max_ctas_per_sm;                                \
         const int grid = total < per_sm * h->num_sms ? total : per_sm * h->num_sms;                                            \
@@ -893,10 +908,11 @@ static int launch_fused(mpcb200_handle* h, int total, int queue_mode, int force_
             CK(cudaMemsetAsync(h->d_smsync, 0, 1024 * 8, h->stream));                                                          \
         }                                                                                                                      \
         CK(cudaMemsetAsync(h->d_queue, 0, 4, h->stream));                                                                      \
-        solve_fused_kernel<LN, EX><<<grid, threads, smem, h->stream>>>(h->cfg, h->L, a);                                       \
+        solve_fused_kernel<LN, EX, WS><<<grid, threads, smem, h->stream>>>(h->cfg, h->L, a);                                   \
     } while (0)
     if (h->has_lines) { if (ext) FUSED_DO(true, true); else FUSED_DO(true, false); }
     else { if (ext) FUSED_DO(false, true); else FUSED_DO(false, false); }
+#undef FUSED_SHAPE
 #undef FUSED_DO
     h->stats.launches_total += 1;
     CK(cudaGetLastError());
