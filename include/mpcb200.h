@@ -436,7 +436,16 @@ int mpcb200_set_stream(mpcb200_handle* h, void* cuda_stream);
    slots needed in the previous batch solve of this handle (a batch costs its slowest instance; a robot that was hard in the last
    cycle tends to be hard in this one).  Order of execution only; 0 = index order. */
 #define MPCB200_OPT_ORDER_BY_HISTORY 6
+/* MPCB200_OPT_FORCE_GENERIC_MODEL: 0 (default) = a unicycle with a point footprint (and no line or moving obstacles, no midpoint
+   differences) runs solve kernels compiled for that model: the robot and footprint tests fold at compile time; 1 = always the
+   kernels that read the model from the configuration.  Both compute the same results bit for bit (A/B comparisons). */
+#define MPCB200_OPT_FORCE_GENERIC_MODEL 7
 int mpcb200_set_option(mpcb200_handle* h, int option, int value);
+/* Model key of the evaluation / line-search code of the last solve launch of this handle: MPCB200_MODEL_GENERIC (also before the
+   first solve) or MPCB200_MODEL_UNI_POINT (compiled for a unicycle with a point footprint, MPCB200_OPT_FORCE_GENERIC_MODEL). */
+#define MPCB200_MODEL_GENERIC 0
+#define MPCB200_MODEL_UNI_POINT 1
+int mpcb200_kernel_model(const mpcb200_handle* h);
 
 /* Counters accumulated since the last mpcb200_stats_reset: kernels launched, device ms per phase. */
 typedef struct mpcb200_stats {

@@ -73,6 +73,23 @@ struct WsLayout
 
 typedef mpcb200_config Cfg;
 
+// ---- robot model / footprint key of a kernel variant ----
+// MODEL_GENERIC reads the robot and footprint model from the configuration at run time.  MODEL_UNI_POINT is compiled for the
+// unicycle with a point footprint (the BASELINE configurations 2, 4 and 5): the tests of the two fields fold at compile time and the
+// code of the other models is not part of the solve kernel, whose iteration is bound by instruction fetch (DESIGN.md section 4).
+#define MODEL_GENERIC MPCB200_MODEL_GENERIC
+#define MODEL_UNI_POINT MPCB200_MODEL_UNI_POINT
+template <int MODEL> struct ModelTraits
+{
+    HD static int robot(const Cfg& c) { return c.robot_type; }
+    HD static int footprint(const Cfg& c) { return c.footprint_type; }
+};
+template <> struct ModelTraits<MODEL_UNI_POINT>
+{
+    HD static constexpr int robot(const Cfg&) { return MPCB200_ROBOT_UNICYCLE; }
+    HD static constexpr int footprint(const Cfg&) { return MPCB200_FOOTPRINT_POINT; }
+};
+
 // ---- elementary functions ----
 HD NOINL inline double normalize_theta_wrap(double theta)
 {
@@ -95,14 +112,16 @@ HD inline double interpolate_angle(double a1, double a2, double factor)
 }
 
 // f(x,u) and derivatives wrt q = (theta, u0, u1): J[j*3+i] = df_j/dq_i, Hc = sum_j nu_j Hess f_j packed (tt,t0,t1,00,01,11)
+template <int MODEL = MODEL_GENERIC>
 HD NOINL inline void dynamics_derivs(const Cfg& c, double th, double v, double w, const double* nu, double* f, double* J,
                                        double* Hc, const double* sc = nullptr)
 {
+    const int robot = ModelTraits<MODEL>::robot(c);
 #pragma unroll
     for (int i = 0; i < 9; ++i) J[i] = 0.0;
 #pragma unroll
     for (int i = 0; i < 6; ++i) Hc[i] = 0.0;
-    if (c.robot_type != MPCB200_ROBOT_KIN_BICYCLE)
+    if (robot != MPCB200_ROBOT_KIN_BICYCLE)
     {
         double s, co;
         if (sc) { s = sc[0]; co = sc[1]; }
@@ -112,11 +131,11 @@ HD NOINL inline void dynamics_derivs(const Cfg& c, double th, double v, double w
         J[3] = v * co; J[4] = s;
         Hc[0] = nu[0] * (-v * co) + nu[1] * (-v * s);
         Hc[1] = nu[0] * (-s) + nu[1] * co;
-        if (c.robot_type == MPCB200_ROBOT_UNICYCLE)
+        if (robot == MPCB200_ROBOT_UNICYCLE)
         {
             f[2] = w; J[8] = 1.0;
         }
-        else if (c.robot_type == MPCB200_ROBOT_SIMPLE_CAR)
+        else if (robot == MPCB200_ROBOT_SIMPLE_CAR)
         {
             const double L = c.wheelbase, t = tan(w), sec2 = 1.0 + t * t;
             f[2] = v * t / L; J[7] = t / L; J[8] = v * sec2 / L;
@@ -178,7 +197,7 @@ HD NOINL inline void dynamics_value(const Cfg& c, double th, double v, double w,
 // distance footprint(pose) <-> point/circle obstacle; optional gradient (x,y,theta) and Hessian (xx,xy,xt,yy,yt,tt)
 // LINES = false compiles the line-obstacle path out (the host knows whether a batch contains line obstacles; the hot
 // kernels are instantiated both ways so that point / circle batches do not pay its registers)
-template <bool WITH_GRAD, bool WITH_HESS, bool LINES = true>
+template <bool WITH_GRAD, bool WITH_HESS, bool LINES = true, int MODEL = MODEL_GENERIC>
 HD inline double footprint_distance_sc(const Cfg& c, double px, double py, double s, double co, int obst_type, const double* op,
                                        double* grad3, double* hess6);
 
@@ -193,17 +212,18 @@ HD inline double footprint_distance(const Cfg& c, double px, double py, double p
 
 // footprint <-> obstacle POINT (wx, wy) (+ obstacle radius r_obst): the point is taken to the robot frame and the closest
 // footprint feature is differentiated through q = R(theta)'(w - p)
-template <bool WITH_GRAD, bool WITH_HESS>
+template <bool WITH_GRAD, bool WITH_HESS, int MODEL = MODEL_GENERIC>
 HD NOINL inline double footprint_distance_point(const Cfg& c, double px, double py, double s, double co, double wx, double wy, double r_obst,
                                           double* grad3, double* hess6)
 {
+    const int footprint = ModelTraits<MODEL>::footprint(c);
     const double ox = wx - px, oy = wy - py;
     const double qx = co * ox + s * oy, qy = -s * ox + co * oy;
     double best = 1e300, bcx = 0, bcy = 0, brho = 0;
     int bvert = 1;
     // iterate the footprint features without materialising the segment list (register pressure)
     int ns;
-    switch (c.footprint_type)
+    switch (footprint)
     {
         case MPCB200_FOOTPRINT_POINT:
         case MPCB200_FOOTPRINT_CIRCULAR:
@@ -214,7 +234,7 @@ HD NOINL inline double footprint_distance_point(const Cfg& c, double px, double 
     for (int i = 0; i < ns; ++i)
     {
         double ax, ay, bx, by, rad = 0.0;
-        switch (c.footprint_type)
+        switch (footprint)
         {
             case MPCB200_FOOTPRINT_POINT: ax = ay = bx = by = 0.0; break;
             case MPCB200_FOOTPRINT_CIRCULAR: ax = ay = bx = by = 0.0; rad = c.footprint_params[0]; break;
@@ -257,17 +277,24 @@ HD NOINL inline double footprint_distance_point(const Cfg& c, double px, double 
         {
             double h00 = 0, h01 = 0, h11 = 0;
             if (bvert) { h00 = (1 - nx * nx) / rho; h01 = -nx * ny / rho; h11 = (1 - ny * ny) / rho; }
-            double H[3][3];
+            // H = J0 (h00 J0 + h01 J1)' + J1 (h01 J0 + h11 J1)' with explicit fused multiply-adds: left to the compiler, the
+            // contraction differed between this loop and its point-footprint form (MODEL_UNI_POINT, the segment folded away), and
+            // with it the Hessian's last bits.  The form is the one the compiler chose for the loop.
+            double a[3], b[3], H[3][3];
+#pragma unroll
+            for (int j = 0; j < 3; ++j) a[j] = fma(h00, J0[j], h01 * J1[j]);
+            b[0] = fma(h11, J1[0], h01 * J0[0]);
+            b[1] = fma(h01, J0[1], h11 * J1[1]);
+            b[2] = fma(h01, J0[2], h11 * J1[2]);
 #pragma unroll
             for (int i = 0; i < 3; ++i)
 #pragma unroll
-                for (int j = 0; j < 3; ++j)
-                    H[i][j] = J0[i] * (h00 * J0[j] + h01 * J1[j]) + J1[i] * (h01 * J0[j] + h11 * J1[j]);
-            double mx = nx * s + ny * co;
+                for (int j = 0; j < 3; ++j) H[i][j] = fma(J0[i], a[j], J1[i] * b[j]);
+            double mx = fma(ny, co, nx * s);
             double my = -nx * co + ny * s;
             H[0][2] += mx; H[2][0] += mx;
             H[1][2] += my; H[2][1] += my;
-            H[2][2] += -(nx * qx + ny * qy);
+            H[2][2] += -fma(qy, ny, qx * nx);
             hess6[0] = H[0][0]; hess6[1] = H[0][1]; hess6[2] = H[0][2];
             hess6[3] = H[1][1]; hess6[4] = H[1][2]; hess6[5] = H[2][2];
         }
@@ -389,12 +416,12 @@ HD NOINL inline double footprint_distance_line(const Cfg& c, double px, double p
 
 // distance footprint(pose) <-> obstacle (point, circle: params x, y, -, -, radius; line: x0, y0, x1, y1) with the sine / cosine of
 // the heading supplied by the caller (one sincos per stage, shared by all rows)
-template <bool WITH_GRAD, bool WITH_HESS, bool LINES>
+template <bool WITH_GRAD, bool WITH_HESS, bool LINES, int MODEL>
 HD inline double footprint_distance_sc(const Cfg& c, double px, double py, double s, double co, int obst_type, const double* op,
                                        double* grad3, double* hess6)
 {
     if (LINES && obst_type == MPCB200_OBST_LINE) return footprint_distance_line<WITH_GRAD, WITH_HESS>(c, px, py, s, co, op, grad3, hess6);
-    return footprint_distance_point<WITH_GRAD, WITH_HESS>(c, px, py, s, co, op[0], op[1], obst_type == MPCB200_OBST_CIRCLE ? op[4] : 0.0, grad3, hess6);
+    return footprint_distance_point<WITH_GRAD, WITH_HESS, MODEL>(c, px, py, s, co, op[0], op[1], obst_type == MPCB200_OBST_CIRCLE ? op[4] : 0.0, grad3, hess6);
 }
 
 // A dynamic obstacle (collision_avoidance/enable_dynamic_obstacles, velocity op[5..6] != 0) enters stage k at the position

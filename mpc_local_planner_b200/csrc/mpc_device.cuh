@@ -474,13 +474,13 @@ __device__ __forceinline__ void evalacc_warp_reduce(EvalAcc& a)
 // ---- PHASE_EVAL (whole CTA, lane per stage): stage functions + derivatives -> condensed KKT records, KKT error,
 //      convergence test (and the time budget: thread 0 reads the clock, sh.fin broadcasts its decision) and barrier update.
 //      Returns 1 (uniform) when the instance terminates. ----
-template <bool LINES>
+template <bool LINES, int MODEL>
 __device__ __forceinline__ int dev_eval(const Cfg& c, const WsLayout& L, double* W, double uprev_dt, CtaShared& sh, int tid, int nt)
 {
     const int N = L.N, lane = tid & 31, wid = tid >> 5, nw = nt >> 5;
     EvalAcc a;
     evalacc_init(a);
-    for (int k = tid; k < N; k += nt) eval_stage<LINES>(c, L, W, W, uprev_dt, k, a);
+    for (int k = tid; k < N; k += nt) eval_stage<LINES, MODEL>(c, L, W, W, uprev_dt, k, a);
     __syncwarp();
     evalacc_warp_reduce(a);
     if (lane == 0) sh.eacc[wid] = a;
@@ -519,7 +519,7 @@ __device__ __forceinline__ void dev_kkt(const Cfg& c, const WsLayout& L, double*
 }
 
 // ---- PHASE_LINESEARCH (whole CTA, lane per stage): step lengths, l1-merit backtracking, iterate update ----
-template <bool LINES>
+template <bool LINES, int MODEL>
 __device__ __forceinline__ void dev_linesearch(const Cfg& c, const WsLayout& L, double* W, double uprev_dt, CtaShared& sh, int tid, int nt)
 {
     const int N = L.N, lane = tid & 31, wid = tid >> 5, nw = nt >> 5;
@@ -577,7 +577,7 @@ __device__ __forceinline__ void dev_linesearch(const Cfg& c, const WsLayout& L, 
     {
         TrialAcc t;
         t.obj = t.inf1 = t.blog = 0.0;
-        for (int k = tid; k < N; k += nt) ls_stage_trial<LINES>(c, L, W, W, uprev_dt, k, alpha, t);
+        for (int k = tid; k < N; k += nt) ls_stage_trial<LINES, MODEL>(c, L, W, W, uprev_dt, k, alpha, t);
         __syncwarp();
         t.obj = warp_sum(t.obj); t.inf1 = warp_sum(t.inf1); t.blog = warp_sum(t.blog);
         if (lane == 0) sh.tr[wid] = t;

@@ -163,8 +163,9 @@ HD inline void lin_rows_component(const Cfg& c, const WsLayout& L, const double*
 
 // Stage functions + derivatives of stage k -> condensed KKT record (G holds the mu-independent part g0, the
 // coefficient of mu is parked in STEP[0..4][k] until the barrier parameter is decided), error accumulators.
-// LINES = false compiles the rarely used obstacle kinds out (line obstacles, moving obstacles): see footprint_distance_sc
-template <bool LINES = true>
+// LINES = false compiles the rarely used obstacle kinds out (line obstacles, moving obstacles): see footprint_distance_sc;
+// MODEL fixes the robot and footprint model at compile time (ModelTraits)
+template <bool LINES = true, int MODEL = MODEL_GENERIC>
 HD inline void eval_stage(const Cfg& c, const WsLayout& L, double* W, double* G, double uprev_dt, int k, EvalAcc& acc)
 {
     const int N = L.N, K = L.K;
@@ -193,8 +194,8 @@ HD inline void eval_stage(const Cfg& c, const WsLayout& L, double* W, double* G,
         // midpoint differences (fd_collocation_se2.h:91-108) evaluate f at the mean heading of the interval; see midpoint_* below
         const bool mid = LINES && is_midpoint(c);
         const double dth = normalize_theta(AX(2, k + 1) - x[2]);
-        if (mid) dynamics_derivs(c, x[2] + 0.5 * dth, u[0], u[1], nu, f, J, Hc, nullptr);
-        else dynamics_derivs(c, x[2], u[0], u[1], nu, f, J, Hc, sc);
+        if (mid) dynamics_derivs<MODEL>(c, x[2] + 0.5 * dth, u[0], u[1], nu, f, J, Hc, nullptr);
+        else dynamics_derivs<MODEL>(c, x[2], u[0], u[1], nu, f, J, Hc, sc);
         e[0] = x[0] + dt * f[0] - AX(0, k + 1);
         e[1] = x[1] + dt * f[1] - AX(1, k + 1);
         e[2] = dt * f[2] - dth;
@@ -389,7 +390,7 @@ HD inline void eval_stage(const Cfg& c, const WsLayout& L, double* W, double* G,
         // midpoint differences: theta_k is also the far end of interval k-1 (weight 1/2 in its mean heading)
         const double nup[3] = {ANU(0, k - 1), ANU(1, k - 1), ANU(2, k - 1)};
         double fp[3], Jp[9], Hp[6];
-        dynamics_derivs(c, AX(2, k - 1) + 0.5 * normalize_theta(x[2] - AX(2, k - 1)), AU(0, k - 1), AU(1, k - 1), nup, fp, Jp, Hp, nullptr);
+        dynamics_derivs<MODEL>(c, AX(2, k - 1) + 0.5 * normalize_theta(x[2] - AX(2, k - 1)), AU(0, k - 1), AU(1, k - 1), nup, fp, Jp, Hp, nullptr);
         const double fx_nu_p = nup[0] * Jp[0] + nup[1] * Jp[3] + nup[2] * Jp[6];
         GL[2] += 0.5 * dt * fx_nu_p;
         H[hidx(2, 2)] += 0.25 * dt * Hp[0];
@@ -424,7 +425,7 @@ HD inline void eval_stage(const Cfg& c, const WsLayout& L, double* W, double* G,
             if (oi < 0) continue;
             double gd[3], hd[6], ob[5];
             const double* op = W + L.oOBST + oi * MPCB200_OBST_STRIDE;
-            const double dist = footprint_distance_sc<true, true, LINES>(c, x[0], x[1], sc[0], sc[1], (int)W[L.oOTYPE + oi],
+            const double dist = footprint_distance_sc<true, true, LINES, MODEL>(c, x[0], x[1], sc[0], sc[1], (int)W[L.oOTYPE + oi],
                                                                   LINES ? obstacle_at(c, op, k, dt, ob) : op, gd, hd);
             const double g = c.min_obstacle_dist - dist;
             const double s = AS(8 + j, k), lam = ALAM(8 + j, k);
@@ -774,7 +775,7 @@ HD NOINL inline double stage_objective(const Cfg& c, const WsLayout& L, const do
 struct TrialAcc { double obj, inf1, blog; };
 // merit pieces of stage k at the trial point z + alpha dz, s + alpha ds.  Linear rows are exact in alpha:
 // g(alpha) + s(alpha) = (1 - alpha) r0, so only the dynamics defect, the objective and the obstacle rows are re-evaluated.
-template <bool LINES = true>
+template <bool LINES = true, int MODEL = MODEL_GENERIC>
 HD inline void ls_stage_trial(const Cfg& c, const WsLayout& L, const double* W, const double* G, double uprev_dt, int k, double alpha, TrialAcc& acc, int part = PART_ALL)
 {
     const int N = L.N, K = L.K;
@@ -789,13 +790,14 @@ HD inline void ls_stage_trial(const Cfg& c, const WsLayout& L, const double* W, 
         const double u[2] = {AU(0, k) + alpha * ASTEP(3, k), AU(1, k) + alpha * ASTEP(4, k)};
         double f[3];
         const double xn2 = AX(2, k + 1) + alpha * ASTEP(2, k + 1);
+        const int robot = ModelTraits<MODEL>::robot(c);
         if (LINES && is_midpoint(c)) dynamics_value(c, x[2] + 0.5 * normalize_theta(xn2 - x[2]), u[0], u[1], f);
-        else if (c.robot_type == MPCB200_ROBOT_KIN_BICYCLE) dynamics_value(c, x[2], u[0], u[1], f);
+        else if (robot == MPCB200_ROBOT_KIN_BICYCLE) dynamics_value(c, x[2], u[0], u[1], f);
         else
         {
             f[0] = u[0] * sc[1]; f[1] = u[0] * sc[0];
-            f[2] = c.robot_type == MPCB200_ROBOT_UNICYCLE ? u[1]
-                 : (c.robot_type == MPCB200_ROBOT_SIMPLE_CAR ? u[0] * tan(u[1]) / c.wheelbase : u[0] * sin(u[1]) / c.wheelbase);
+            f[2] = robot == MPCB200_ROBOT_UNICYCLE ? u[1]
+                 : (robot == MPCB200_ROBOT_SIMPLE_CAR ? u[0] * tan(u[1]) / c.wheelbase : u[0] * sin(u[1]) / c.wheelbase);
         }
         const double xn[3] = {AX(0, k + 1) + alpha * ASTEP(0, k + 1), AX(1, k + 1) + alpha * ASTEP(1, k + 1),
                               AX(2, k + 1) + alpha * ASTEP(2, k + 1)};
@@ -822,7 +824,7 @@ HD inline void ls_stage_trial(const Cfg& c, const WsLayout& L, const double* W, 
             const int oi = (int)AOBS(j, k);
             if (oi < 0) continue;
             double ob[5];
-            const double dist = footprint_distance_sc<false, false, LINES>(c, x[0], x[1], sc[0], sc[1], (int)W[L.oOTYPE + oi],
+            const double dist = footprint_distance_sc<false, false, LINES, MODEL>(c, x[0], x[1], sc[0], sc[1], (int)W[L.oOTYPE + oi],
                                                                     LINES ? obstacle_at(c, W + L.oOBST + oi * MPCB200_OBST_STRIDE, k, dtt, ob) : W + L.oOBST + oi * MPCB200_OBST_STRIDE,
                                                                     nullptr, nullptr);
             double sn = AS(8 + j, k) + alpha * ADS(8 + j, k);

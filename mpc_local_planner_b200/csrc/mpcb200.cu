@@ -81,7 +81,7 @@ __device__ __forceinline__ void mark_invalid(const WsLayout& L, double* W)
 }
 
 // ---- kernel: ONE PHASE of the solve for every instance of a batch (kernel-level API and the phased solve mode) ----
-template <bool LINES>
+template <bool LINES, int MODEL>
 __global__ void __launch_bounds__(MAX_GROUP_WARPS * 32, 3) phase_kernel(const __grid_constant__ Cfg c, const __grid_constant__ WsLayout L, double* ws, int B, int phase,
                                                                        double uprev_dt, int force_cold, int first_outer, int* n_active, int img_words, InputPtrs in)
 {
@@ -116,11 +116,11 @@ __global__ void __launch_bounds__(MAX_GROUP_WARPS * 32, 3) phase_kernel(const __
             break;
         case MPCB200_PHASE_EVAL:
         {
-            const int fin = dev_eval<LINES>(c, L, W, uprev_dt, sh, tid, nt);
+            const int fin = dev_eval<LINES, MODEL>(c, L, W, uprev_dt, sh, tid, nt);
             if (!fin && n_active && tid == 0) atomicAdd(n_active, 1);
             break;
         }
-        case MPCB200_PHASE_LINESEARCH: dev_linesearch<LINES>(c, L, W, uprev_dt, sh, tid, nt); break;
+        case MPCB200_PHASE_LINESEARCH: dev_linesearch<LINES, MODEL>(c, L, W, uprev_dt, sh, tid, nt); break;
         default: break;
     }
     // everything but the inputs -- except after the association over a long list, which fills the resident obstacles
@@ -291,7 +291,7 @@ template <int WARPS> struct FusedShape;
 template <> struct FusedShape<SMALL_GROUP_WARPS> { static constexpr int MIN_CTAS = 4; };
 template <> struct FusedShape<MAX_GROUP_WARPS> { static constexpr int MIN_CTAS = 2; };
 
-template <bool LINES, bool EXT, int WARPS>
+template <bool LINES, bool EXT, int WARPS, int MODEL>
 __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve_fused_kernel(const __grid_constant__ Cfg c, const __grid_constant__ WsLayout L, const __grid_constant__ FusedArgs a)
 {
     extern __shared__ __align__(128) unsigned char dyn_smem[];
@@ -372,7 +372,7 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
                 for (;;)
                 {
                     if (nph == 3u) PHASE_GATE(0u);
-                    const int fin = dev_eval<LINES>(c, L, W, a.uprev_dt, sh, tid, nt);
+                    const int fin = dev_eval<LINES, MODEL>(c, L, W, a.uprev_dt, sh, tid, nt);
                     TICK(MPCB200_PHASE_EVAL);
                     if (fin) break;
                     PHASE_GATE(nph - 2u);
@@ -382,7 +382,7 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
                     ++n_kkt;
                     if (ASC(MPCB200_SC_STATUS) >= 0.0) break;   // inertia correction failed: given up
                     PHASE_GATE(nph - 1u);
-                    dev_linesearch<LINES>(c, L, W, a.uprev_dt, sh, tid, nt);
+                    dev_linesearch<LINES, MODEL>(c, L, W, a.uprev_dt, sh, tid, nt);
                     TICK(MPCB200_PHASE_LINESEARCH);
                     if (ASC(MPCB200_SC_STATUS) >= 0.0) break;   // jammed: given up
                 }
@@ -507,6 +507,8 @@ struct mpcb200_handle
     int sm_phase_sync;    // MPCB200_OPT_SM_PHASE_SYNC: co-resident CTAs of the solve kernel enter the phases together
     unsigned long long* d_smsync;
     int max_ctas_per_sm;  // MPCB200_OPT_CTAS_PER_SM: cap on the resident CTAs per SM of the solve kernel (0 = what fits)
+    int force_generic_model;  // MPCB200_OPT_FORCE_GENERIC_MODEL: never launch the variants compiled for one robot / footprint model
+    int last_model;           // model key of the last solve launch (mpcb200_kernel_model)
     mpcb200_stats stats;
     std::vector<cudaEvent_t> ev;  // pool of event pairs
     std::vector<int> ev_phase;
@@ -610,7 +612,7 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
     make_layout(cfg, MAX_OBST, MAX_VP, h->L);
     h->n_cap = cfg->n; h->d_resample = nullptr; h->d_cm = nullptr; h->cm_cap = 0; h->costmap_ms = 0.0; h->d_fz = nullptr; h->fz_cap = 0;
     h->uprev_dt = 0.0; h->has_obst = h->has_vp = h->has_xinit = h->has_reinit = 0; h->obst_max = h->vp_max = 0; h->has_lines = 0;
-    h->solve_mode = 0; h->timing_mask = 1u << MPCB200_PHASE_KKT; h->fused_grid = 0; h->max_ctas_per_sm = 0; h->sm_phase_sync = -1; h->d_smsync = nullptr; h->order_by_history = 1; h->hist_B = 0; h->d_prev_iters = h->d_prev_status = h->d_order = nullptr;
+    h->solve_mode = 0; h->timing_mask = 1u << MPCB200_PHASE_KKT; h->fused_grid = 0; h->max_ctas_per_sm = 0; h->force_generic_model = 0; h->last_model = MODEL_GENERIC; h->sm_phase_sync = -1; h->d_smsync = nullptr; h->order_by_history = 1; h->hist_B = 0; h->d_prev_iters = h->d_prev_status = h->d_order = nullptr;
     h->d_origin = nullptr;
     // seconds -> ns, rounded up; a budget beyond 2^62 ns (146 years) is no budget
     h->budget_ns = (cfg->max_cpu_time > 0.0 && cfg->max_cpu_time * 1e9 < 4611686018427387904.0) ? (unsigned long long)ceil(cfg->max_cpu_time * 1e9) : 0ull;
@@ -638,11 +640,13 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
     CKC(cudaMalloc(&h->d_status, B * 4)); CKC(cudaMalloc(&h->d_iters, B * 4)); CKC(cudaMalloc(&h->d_nactive, 8)); CKC(cudaMalloc(&h->d_queue, 4)); CKC(cudaMalloc(&h->d_smsync, 1024 * 8)); CKC(cudaMalloc(&h->d_prev_iters, B * 4)); CKC(cudaMalloc(&h->d_prev_status, B * 4)); CKC(cudaMalloc(&h->d_order, B * 4));
     CKC(cudaMalloc(&h->d_origin, 8));
     CKC(cudaMalloc(&h->d_counters, CNT_WORDS * 8)); CKC(cudaMemsetAsync(h->d_counters, 0, CNT_WORDS * 8, h->stream));
-    CKC(allow_smem(phase_kernel<false>)); CKC(allow_smem(phase_kernel<true>));
+    CKC(allow_smem(phase_kernel<false, MODEL_GENERIC>)); CKC(allow_smem(phase_kernel<true, MODEL_GENERIC>));
+    CKC(allow_smem(phase_kernel<false, MODEL_UNI_POINT>));
     CKC(allow_smem(kkt_warp_kernel<false>)); CKC(allow_smem(kkt_warp_kernel<true>));
-#define ALLOW_FUSED(W_)                                                                                              \
-    CKC(allow_smem(solve_fused_kernel<false, false, W_>)); CKC(allow_smem(solve_fused_kernel<false, true, W_>));     \
-    CKC(allow_smem(solve_fused_kernel<true, false, W_>)); CKC(allow_smem(solve_fused_kernel<true, true, W_>))
+#define ALLOW_FUSED(W_)                                                                                                                  \
+    CKC(allow_smem(solve_fused_kernel<false, false, W_, MODEL_GENERIC>)); CKC(allow_smem(solve_fused_kernel<false, true, W_, MODEL_GENERIC>)); \
+    CKC(allow_smem(solve_fused_kernel<true, false, W_, MODEL_GENERIC>)); CKC(allow_smem(solve_fused_kernel<true, true, W_, MODEL_GENERIC>));   \
+    CKC(allow_smem(solve_fused_kernel<false, false, W_, MODEL_UNI_POINT>)); CKC(allow_smem(solve_fused_kernel<false, true, W_, MODEL_UNI_POINT>))
     ALLOW_FUSED(SMALL_GROUP_WARPS);
     ALLOW_FUSED(MAX_GROUP_WARPS);
 #undef ALLOW_FUSED
@@ -726,6 +730,13 @@ static int group_threads(const mpcb200_handle* h)
     const int gw = (h->cfg.n + 31) / 32;
     return 32 * (gw < MAX_GROUP_WARPS ? gw : MAX_GROUP_WARPS);   // a lane per stage
 }
+// robot model / footprint key of the evaluation and line-search code a launch runs (ModelTraits).  The specialised variants exist for
+// the kernels without the rarely used obstacle paths only (LINES = false).
+static int kernel_model(const mpcb200_handle* h)
+{
+    const bool uni_point = h->cfg.robot_type == MPCB200_ROBOT_UNICYCLE && h->cfg.footprint_type == MPCB200_FOOTPRINT_POINT;
+    return (uni_point && !h->has_lines && !h->force_generic_model) ? MODEL_UNI_POINT : MODEL_GENERIC;
+}
 static int image_words(const mpcb200_handle* h) { return resident_words(h->L, h->has_obst ? (h->obst_max < h->L.M ? h->obst_max : h->L.M) : 0); }
 
 static InputPtrs batch_inputs(mpcb200_handle* h, bool with_uprev);
@@ -742,8 +753,12 @@ static int launch_phase(mpcb200_handle* h, int phase, int B, int force_cold, int
     }
     else if (phase >= 0 && phase < MPCB200_NUM_PHASES)
     {
-        if (h->has_lines) phase_kernel<true><<<B, group_threads(h), img_smem, h->stream>>>(h->cfg, h->L, h->ws, B, phase, h->uprev_dt, force_cold, first_outer, n_active, img_words, batch_inputs(h, true));
-        else phase_kernel<false><<<B, group_threads(h), img_smem, h->stream>>>(h->cfg, h->L, h->ws, B, phase, h->uprev_dt, force_cold, first_outer, n_active, img_words, batch_inputs(h, true));
+#define PHASE_DO(LN, MD) phase_kernel<LN, MD><<<B, group_threads(h), img_smem, h->stream>>>(h->cfg, h->L, h->ws, B, phase, h->uprev_dt, force_cold, first_outer, n_active, img_words, batch_inputs(h, true))
+        if (h->has_lines) PHASE_DO(true, MODEL_GENERIC);
+        else if (kernel_model(h) == MODEL_UNI_POINT) PHASE_DO(false, MODEL_UNI_POINT);
+        else PHASE_DO(false, MODEL_GENERIC);
+        h->last_model = kernel_model(h);
+#undef PHASE_DO
     }
     else return set_err(h, MPCB200_E_INVALID, "unknown phase");
     if (timed) ev_end(h);
@@ -893,10 +908,10 @@ static int launch_fused(mpcb200_handle* h, int total, int queue_mode, int force_
     const int threads = group_threads(h);
     const bool ext = kkt_is_ext(h->cfg), small = threads <= SMALL_GROUP_WARPS * 32;
     int per_sm = 0;
-#define FUSED_DO(LN, EX) do { if (small) FUSED_SHAPE(LN, EX, SMALL_GROUP_WARPS); else FUSED_SHAPE(LN, EX, MAX_GROUP_WARPS); } while (0)
-#define FUSED_SHAPE(LN, EX, WS)                                                                                                \
+#define FUSED_DO(LN, EX, MD) do { if (small) FUSED_SHAPE(LN, EX, SMALL_GROUP_WARPS, MD); else FUSED_SHAPE(LN, EX, MAX_GROUP_WARPS, MD); } while (0)
+#define FUSED_SHAPE(LN, EX, WS, MD)                                                                                            \
     do {                                                                                                                       \
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, solve_fused_kernel<LN, EX, WS>, threads, smem));             \
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, solve_fused_kernel<LN, EX, WS, MD>, threads, smem));         \
         if (per_sm < 1) return set_err(h, MPCB200_E_UNSUPPORTED, "the solve kernel does not fit on an SM with this configuration"); \
         if (h->max_ctas_per_sm > 0 && per_sm > h->max_ctas_per_sm) per_sm = h->max_ctas_per_sm;                                \
         const int grid = total < per_sm * h->num_sms ? total : per_sm * h->num_sms;                                            \
@@ -908,10 +923,12 @@ static int launch_fused(mpcb200_handle* h, int total, int queue_mode, int force_
             CK(cudaMemsetAsync(h->d_smsync, 0, 1024 * 8, h->stream));                                                          \
         }                                                                                                                      \
         CK(cudaMemsetAsync(h->d_queue, 0, 4, h->stream));                                                                      \
-        solve_fused_kernel<LN, EX, WS><<<grid, threads, smem, h->stream>>>(h->cfg, h->L, a);                                   \
+        solve_fused_kernel<LN, EX, WS, MD><<<grid, threads, smem, h->stream>>>(h->cfg, h->L, a);                               \
     } while (0)
-    if (h->has_lines) { if (ext) FUSED_DO(true, true); else FUSED_DO(true, false); }
-    else { if (ext) FUSED_DO(false, true); else FUSED_DO(false, false); }
+    if (h->has_lines) { if (ext) FUSED_DO(true, true, MODEL_GENERIC); else FUSED_DO(true, false, MODEL_GENERIC); }
+    else if (kernel_model(h) == MODEL_UNI_POINT) { if (ext) FUSED_DO(false, true, MODEL_UNI_POINT); else FUSED_DO(false, false, MODEL_UNI_POINT); }
+    else { if (ext) FUSED_DO(false, true, MODEL_GENERIC); else FUSED_DO(false, false, MODEL_GENERIC); }
+    h->last_model = kernel_model(h);
 #undef FUSED_SHAPE
 #undef FUSED_DO
     h->stats.launches_total += 1;
@@ -1291,8 +1308,11 @@ extern "C" int mpcb200_set_option(mpcb200_handle* h, int option, int value)
     if (option == MPCB200_OPT_CTAS_PER_SM && value >= 0 && value <= 32) { h->max_ctas_per_sm = value; return 0; }
     if (option == MPCB200_OPT_ORDER_BY_HISTORY && value >= 0 && value <= 1) { h->order_by_history = value; return 0; }
     if (option == MPCB200_OPT_SM_PHASE_SYNC && value >= -1 && value <= 2) { h->sm_phase_sync = value; return 0; }
+    if (option == MPCB200_OPT_FORCE_GENERIC_MODEL && value >= 0 && value <= 1) { h->force_generic_model = value; return 0; }
     return set_err(h, MPCB200_E_INVALID, "unknown option or value");
 }
+
+extern "C" int mpcb200_kernel_model(const mpcb200_handle* h) { return h ? h->last_model : MPCB200_E_INVALID; }
 
 extern "C" int mpcb200_set_timing(mpcb200_handle* h, unsigned phase_mask)
 {
