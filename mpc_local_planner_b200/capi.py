@@ -185,6 +185,12 @@ def pack_viapoints(count, poses):
     return v, (count, poses)
 
 
+def result_arrays(B, N):
+    """Host arrays for the results of B instances at horizon N, in the layout the solve entry points write."""
+    return dict(u_seq=np.empty((B, N, 2)), x_seq=np.empty((B, N, 3)), dt=np.empty(B),
+                status=np.empty(B, dtype=np.int32), kkt_err=np.empty(B), iters=np.empty(B, dtype=np.int32))
+
+
 _LIB = None
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG_DIR, "libmpcb200.so")
@@ -325,9 +331,7 @@ class BatchSolver:
     def solve_stream(self, x0, xf, u_prev=None, u_prev_dt=0.0, obstacles=None, viapoints=None):
         """A queue of len(x0) instances (any number) through the pool of max_batch slots: continuous batching, cold starts."""
         T, x0, xf, u_prev, o, v, xi, keep = self._prep_inputs(x0, xf, u_prev, obstacles, viapoints, None)
-        N = self.N
-        out = dict(u_seq=np.empty((T, N, 2)), x_seq=np.empty((T, N, 3)), dt=np.empty(T),
-                   status=np.empty(T, dtype=np.int32), kkt_err=np.empty(T), iters=np.empty(T, dtype=np.int32))
+        out = result_arrays(T, self.N)
         t = C.c_double(0.0)
         rc = self.lib.mpcb200_solve_stream(
             self.h, T, _dp(x0), _dp(xf), _dp(u_prev), float(u_prev_dt), C.byref(o) if o else None, C.byref(v) if v else None,
@@ -339,9 +343,7 @@ class BatchSolver:
     def alloc_outputs(self, B, pin=None):
         """Result buffers for step(..., out=...).  pin: optional callable array -> (pinned array, owner) (e.g. through
         torch.Tensor.pin_memory): page-locked buffers take the device-to-host copies without a staging copy."""
-        N = self.N
-        out = dict(u_seq=np.empty((B, N, 2)), x_seq=np.empty((B, N, 3)), dt=np.empty(B),
-                   status=np.empty(B, dtype=np.int32), kkt_err=np.empty(B), iters=np.empty(B, dtype=np.int32))
+        out = result_arrays(B, self.N)
         if pin is not None:
             owners = []
             for k in list(out):
@@ -384,9 +386,7 @@ class BatchSolver:
         return t.value
 
     def fetch(self):
-        B, N = self.B, self.N
-        out = dict(u_seq=np.empty((B, N, 2)), x_seq=np.empty((B, N, 3)), dt=np.empty(B),
-                   status=np.empty(B, dtype=np.int32), kkt_err=np.empty(B), iters=np.empty(B, dtype=np.int32))
+        out = result_arrays(self.B, self.N)
         rc = self.lib.mpcb200_fetch_results(self.h, _dp(out["u_seq"]), _dp(out["x_seq"]), _dp(out["dt"]),
                                             _ip(out["status"]), _dp(out["kkt_err"]), _ip(out["iters"]))
         self._check(rc, "mpcb200_fetch_results")
@@ -554,9 +554,7 @@ class MultiSolver:
 
     def step(self, x0, xf, u_prev=None, u_prev_dt=0.0, obstacles=None, viapoints=None):
         B, x0, xf, u_prev, o, v, xi, keep = BatchSolver._prep_inputs(x0, xf, u_prev, obstacles, viapoints, None)
-        N = self.N
-        out = dict(u_seq=np.empty((B, N, 2)), x_seq=np.empty((B, N, 3)), dt=np.empty(B),
-                   status=np.empty(B, dtype=np.int32), kkt_err=np.empty(B), iters=np.empty(B, dtype=np.int32))
+        out = result_arrays(B, self.N)
         t = C.c_double(0.0)
         rc = self.lib.mpcb200_step_batch_multi(
             self.h, B, _dp(x0), _dp(xf), _dp(u_prev), float(u_prev_dt), C.byref(o) if o else None, C.byref(v) if v else None, None, None,

@@ -466,53 +466,60 @@ __global__ void flush_kernel(double* buf, size_t n)
 // =================================================================================================================
 // host side
 // =================================================================================================================
+// Compact device arrays of the inputs and outputs of `rows` instances: the batch's (instance i <-> block i) and the queue job's
+// (mpcb200_solve_stream).  `in`, `uprev_dt` and `has_lines` describe what load_inputs last put in them: the launches on these
+// arrays read nothing else.
+struct IoBuffers
+{
+    size_t rows = 0;     // instances the arrays hold
+    int obst_m = 0;      // obstacles per instance the obstacle arrays hold
+    double *x0 = nullptr, *xf = nullptr, *uprev = nullptr, *obst = nullptr, *vp = nullptr, *xinit = nullptr;
+    int *obst_count = nullptr, *obst_type = nullptr, *vp_count = nullptr;
+    unsigned char* reinit = nullptr;
+    double *useq = nullptr, *xseq = nullptr, *dt = nullptr, *kkt = nullptr, *upacked = nullptr;
+    int *status = nullptr, *iters = nullptr;
+    InputPtrs in{};
+    double uprev_dt = 0.0;
+    int has_lines = 0;   // line obstacles, moving obstacles or midpoint differences: the kernel variants with those (rarely used) paths
+    OutputPtrs out() const { return OutputPtrs{useq, xseq, dt, status, kkt, iters, upacked}; }
+};
+
 struct mpcb200_handle
 {
-    Cfg cfg;
-    WsLayout L;
-    int max_batch, device, B;
-    int n_cap;                  // horizon the buffers were sized for at create (mpcb200_resample moves cfg.n within [3, n_cap])
-    double* d_resample;         // scratch of mpcb200_resample, allocated on first use
-    void* d_cm; size_t cm_cap; double costmap_ms;
-    void* d_fz; size_t fz_cap;   // scratch of mpcb200_check_feasible (maps, trajectories, footprint, flags)  // scratch of mpcb200_costmap_obstacles (grown on demand), device ms of its last call
-    double* ws;
-    int num_sms, clock_khz;
-    int solve_mode;             // MPCB200_OPT_SOLVE_MODE: 0 fused persistent kernel (default), 1 one kernel per phase
-    unsigned timing_mask;       // phased mode: phases bracketed by CUDA events inside solve (bit = phase id)
-    cudaStream_t stream, own_stream;  // stream in use / the stream the handle created
-    // compact device input / output staging
-    double *d_x0, *d_xf, *d_uprev, *d_obst, *d_vp, *d_xinit;
-    int *d_obst_count, *d_obst_type, *d_vp_count;
-    unsigned char* d_reinit;
-    double *d_useq, *d_xseq, *d_dt, *d_kkt, *d_upacked;
-    int *d_status, *d_iters, *d_nactive, *d_queue;
-    unsigned long long* d_counters;
-    int* h_nactive;  // pinned, two poll slots
-    cudaEvent_t poll_ev[2], t0, t1, c0, c1;   // t: around a solve, c: around the costmap kernels
-    double* d_flush; size_t flush_n;
-    int has_obst, has_vp, has_xinit, has_reinit, obst_max, vp_max;
-    int d_obst_m, s_obst_m;   // obstacles per instance the staging arrays (batch / queue job) hold
-    // queue job (mpcb200_solve_stream): inputs / outputs of the whole queue on the device (grown on demand)
-    size_t stream_cap;
-    double *s_x0, *s_xf, *s_uprev, *s_obst, *s_vp, *s_useq, *s_xseq, *s_dt, *s_kkt, *s_upacked;
-    int *s_obst_count, *s_obst_type, *s_vp_count, *s_status, *s_iters;
-    int has_lines;  // line obstacles in the batch, moving obstacles or midpoint differences: the kernels are launched with those (rarely used) paths compiled in
-    double uprev_dt;
-    int fused_grid;  // CTAs of the last fused launch
-    int order_by_history; // MPCB200_OPT_ORDER_BY_HISTORY: batch queue longest-first by the previous solve's iteration counts
-    int hist_B;           // batch size of the last batch solve whose iteration counts are in d_iters (0: none)
-    int *d_prev_iters, *d_prev_status, *d_order;
-    unsigned long long budget_ns;   // max_cpu_time in ns (0: no budget)
-    unsigned long long* d_origin;   // start of the current solve launch (%globaltimer), see FusedArgs
-    int sm_phase_sync;    // MPCB200_OPT_SM_PHASE_SYNC: co-resident CTAs of the solve kernel enter the phases together
-    unsigned long long* d_smsync;
-    int max_ctas_per_sm;  // MPCB200_OPT_CTAS_PER_SM: cap on the resident CTAs per SM of the solve kernel (0 = what fits)
-    int force_generic_model;  // MPCB200_OPT_FORCE_GENERIC_MODEL: never launch the variants compiled for one robot / footprint model
-    int last_model;           // model key of the last solve launch (mpcb200_kernel_model)
-    mpcb200_stats stats;
-    std::vector<cudaEvent_t> ev;  // pool of event pairs
+    Cfg cfg{};
+    WsLayout L{};
+    int max_batch = 0, device = 0, B = 0;
+    int n_cap = 0;                   // horizon the buffers were sized for at create (mpcb200_resample moves cfg.n within [3, n_cap])
+    double* d_resample = nullptr;    // scratch of mpcb200_resample, allocated on first use
+    void* d_cm = nullptr; size_t cm_cap = 0; double costmap_ms = 0.0;   // scratch of mpcb200_costmap_obstacles (grown on demand), device ms of its last call
+    void* d_fz = nullptr; size_t fz_cap = 0;   // scratch of mpcb200_check_feasible (maps, trajectories, footprint, flags)
+    double* ws = nullptr;
+    int num_sms = 0, clock_khz = 0;
+    int solve_mode = 0;              // MPCB200_OPT_SOLVE_MODE: 0 fused persistent kernel (default), 1 one kernel per phase
+    unsigned timing_mask = 1u << MPCB200_PHASE_KKT;   // phased mode: phases bracketed by CUDA events inside solve (bit = phase id)
+    cudaStream_t stream = nullptr, own_stream = nullptr;   // stream in use / the stream the handle created
+    IoBuffers batch;                 // sized for max_batch at create
+    IoBuffers queue;                 // the queue job's: inputs / outputs of the whole queue (grown on demand)
+    int *d_nactive = nullptr, *d_queue = nullptr;
+    unsigned long long* d_counters = nullptr;
+    int* h_nactive = nullptr;        // pinned, two poll slots
+    cudaEvent_t poll_ev[2] = {nullptr, nullptr}, t0 = nullptr, t1 = nullptr, c0 = nullptr, c1 = nullptr;   // t: around a solve, c: around the costmap kernels
+    double* d_flush = nullptr; size_t flush_n = 0;
+    int fused_grid = 0;              // CTAs of the last fused launch
+    int order_by_history = 1;        // MPCB200_OPT_ORDER_BY_HISTORY: batch queue longest-first by the previous solve's iteration counts
+    int hist_B = 0;                  // batch size of the last batch solve whose iteration counts are in batch.iters (0: none)
+    int *d_prev_iters = nullptr, *d_prev_status = nullptr, *d_order = nullptr;
+    unsigned long long budget_ns = 0;          // max_cpu_time in ns (0: no budget)
+    unsigned long long* d_origin = nullptr;    // start of the current solve launch (%globaltimer), see FusedArgs
+    int sm_phase_sync = -1;          // MPCB200_OPT_SM_PHASE_SYNC: co-resident CTAs of the solve kernel enter the phases together
+    unsigned long long* d_smsync = nullptr;
+    int max_ctas_per_sm = 0;         // MPCB200_OPT_CTAS_PER_SM: cap on the resident CTAs per SM of the solve kernel (0 = what fits)
+    int force_generic_model = 0;     // MPCB200_OPT_FORCE_GENERIC_MODEL: never launch the variants compiled for one robot / footprint model
+    int last_model = MODEL_GENERIC;  // model key of the last solve launch (mpcb200_kernel_model)
+    mpcb200_stats stats{};
+    std::vector<cudaEvent_t> ev;     // pool of event pairs
     std::vector<int> ev_phase;
-    size_t ev_used;
+    size_t ev_used = 0;
     std::string err;
 };
 
@@ -594,6 +601,67 @@ static int validate_config(const mpcb200_config* c, std::string& why)
 template <class K>
 static cudaError_t allow_smem(K kernel) { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_IMG_SMEM); }
 
+// ---- the kernel variants: one table per kernel.  The variants compiled for one robot / footprint model (MODEL_UNI_POINT) exist
+//      without the line-obstacle paths only (LINES = false); a request for one with them gets the generic variant. ----
+using FusedKernel = decltype(&solve_fused_kernel<false, false, SMALL_GROUP_WARPS, MODEL_GENERIC>);
+template <int WARPS>
+static FusedKernel fused_shape_variant(bool lines, bool ext, int model)
+{
+    if (lines) return ext ? solve_fused_kernel<true, true, WARPS, MODEL_GENERIC> : solve_fused_kernel<true, false, WARPS, MODEL_GENERIC>;
+    if (model == MODEL_UNI_POINT) return ext ? solve_fused_kernel<false, true, WARPS, MODEL_UNI_POINT> : solve_fused_kernel<false, false, WARPS, MODEL_UNI_POINT>;
+    return ext ? solve_fused_kernel<false, true, WARPS, MODEL_GENERIC> : solve_fused_kernel<false, false, WARPS, MODEL_GENERIC>;
+}
+static FusedKernel fused_variant(bool lines, bool ext, bool small, int model)
+{
+    return small ? fused_shape_variant<SMALL_GROUP_WARPS>(lines, ext, model) : fused_shape_variant<MAX_GROUP_WARPS>(lines, ext, model);
+}
+using PhaseKernel = decltype(&phase_kernel<false, MODEL_GENERIC>);
+static PhaseKernel phase_variant(bool lines, int model)
+{
+    if (lines) return phase_kernel<true, MODEL_GENERIC>;
+    return model == MODEL_UNI_POINT ? phase_kernel<false, MODEL_UNI_POINT> : phase_kernel<false, MODEL_GENERIC>;
+}
+
+// frees the arrays of `io` and empties it (nothing held)
+static void io_release(IoBuffers& io)
+{
+    void* arrays[] = {io.x0, io.xf, io.uprev, io.obst, io.vp, io.xinit, io.obst_count, io.obst_type, io.vp_count, io.reinit,
+                      io.useq, io.xseq, io.dt, io.kkt, io.upacked, io.status, io.iters};
+    for (void* p : arrays) cudaFree(p);   // (no-op for the null ones)
+    io = IoBuffers{};
+}
+// Grows `io` to hold `rows` instances and `obst_per_instance` obstacles per instance (at least MAX_OBST: longer lists get arrays
+// of their length on first use).  Only the obstacle arrays move when only the obstacle list grows, so the outputs of the last
+// solve stay where they are.  Rows are sized for the largest horizon the handle can be resampled to.  x_init / reinit: the
+// batch only (the queue's instances start cold).
+static int io_reserve(mpcb200_handle* h, IoBuffers& io, size_t rows, int obst_per_instance)
+{
+    const int m = (obst_per_instance > MAX_OBST && obst_per_instance <= MAX_OBST_LIST) ? obst_per_instance : MAX_OBST;
+    if (rows <= io.rows && m <= io.obst_m) return 0;
+    CK(cudaStreamSynchronize(h->stream));   // work queued on the stream may still read the arrays
+    if (rows > io.rows)
+    {
+        io_release(io);
+        const size_t T = rows, N = (size_t)h->n_cap;
+        CK(cudaMalloc(&io.x0, T * 3 * 8)); CK(cudaMalloc(&io.xf, T * 3 * 8)); CK(cudaMalloc(&io.uprev, T * 2 * 8));
+        CK(cudaMalloc(&io.obst_count, T * 4)); CK(cudaMalloc(&io.vp, T * MAX_VP * 3 * 8)); CK(cudaMalloc(&io.vp_count, T * 4));
+        if (&io == &h->batch) { CK(cudaMalloc(&io.xinit, T * N * 3 * 8)); CK(cudaMalloc(&io.reinit, T)); }
+        CK(cudaMalloc(&io.useq, T * N * 2 * 8)); CK(cudaMalloc(&io.xseq, T * N * 3 * 8)); CK(cudaMalloc(&io.dt, T * 8));
+        CK(cudaMalloc(&io.kkt, T * 8)); CK(cudaMalloc(&io.upacked, T * (N - 1) * 2 * 8));
+        CK(cudaMalloc(&io.status, T * 4)); CK(cudaMalloc(&io.iters, T * 4));
+        io.rows = rows;
+    }
+    if (m > io.obst_m)
+    {
+        cudaFree(io.obst); cudaFree(io.obst_type);
+        io.obst = nullptr; io.obst_type = nullptr; io.obst_m = 0;
+        CK(cudaMalloc(&io.obst, io.rows * m * MPCB200_OBST_STRIDE * 8));
+        CK(cudaMalloc(&io.obst_type, io.rows * m * 4));
+        io.obst_m = m;
+    }
+    return 0;
+}
+
 extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int device, mpcb200_handle** out)
 {
     mpcb200_handle* h = nullptr;
@@ -607,53 +675,41 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
         return set_err(nullptr, MPCB200_E_NODEVICE, std::string("no CUDA device (") + cudaGetErrorString(e) + "): this solver has no CPU fallback");
     if (device < 0 || device >= ndev) return set_err(nullptr, MPCB200_E_INVALID, "device index out of range");
     h = new mpcb200_handle();
-    h->cfg = *cfg; h->max_batch = max_batch; h->device = device; h->B = 0; h->ws = nullptr; h->ev_used = 0;
-    memset(&h->stats, 0, sizeof(h->stats));
+    h->cfg = *cfg; h->max_batch = max_batch; h->device = device; h->n_cap = cfg->n;
     make_layout(cfg, MAX_OBST, MAX_VP, h->L);
-    h->n_cap = cfg->n; h->d_resample = nullptr; h->d_cm = nullptr; h->cm_cap = 0; h->costmap_ms = 0.0; h->d_fz = nullptr; h->fz_cap = 0;
-    h->uprev_dt = 0.0; h->has_obst = h->has_vp = h->has_xinit = h->has_reinit = 0; h->obst_max = h->vp_max = 0; h->has_lines = 0;
-    h->solve_mode = 0; h->timing_mask = 1u << MPCB200_PHASE_KKT; h->fused_grid = 0; h->max_ctas_per_sm = 0; h->force_generic_model = 0; h->last_model = MODEL_GENERIC; h->sm_phase_sync = -1; h->d_smsync = nullptr; h->order_by_history = 1; h->hist_B = 0; h->d_prev_iters = h->d_prev_status = h->d_order = nullptr;
-    h->d_origin = nullptr;
     // seconds -> ns, rounded up; a budget beyond 2^62 ns (146 years) is no budget
     h->budget_ns = (cfg->max_cpu_time > 0.0 && cfg->max_cpu_time * 1e9 < 4611686018427387904.0) ? (unsigned long long)ceil(cfg->max_cpu_time * 1e9) : 0ull;
 #define CKC(call)                                                                                                  \
     do {                                                                                                           \
         cudaError_t e_ = (call);                                                                                   \
-        if (e_ != cudaSuccess) { std::string m = std::string(#call) + ": " + cudaGetErrorString(e_); delete h; return set_err(nullptr, MPCB200_E_CUDA, m); } \
+        if (e_ != cudaSuccess) { std::string m = std::string(#call) + ": " + cudaGetErrorString(e_); mpcb200_destroy(h); return set_err(nullptr, MPCB200_E_CUDA, m); } \
     } while (0)
     CKC(cudaSetDevice(device));
     CKC(cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking));
     h->stream = h->own_stream;
-    const size_t B = (size_t)max_batch, N = (size_t)cfg->n;
+    const size_t B = (size_t)max_batch;
     CKC(cudaMalloc(&h->ws, B * h->L.stride * sizeof(double)));
     CKC(cudaMemsetAsync(h->ws, 0, B * h->L.stride * sizeof(double), h->stream));
     CKC(cudaDeviceGetAttribute(&h->num_sms, cudaDevAttrMultiProcessorCount, device));
     CKC(cudaDeviceGetAttribute(&h->clock_khz, cudaDevAttrClockRate, device));
-    CKC(cudaMalloc(&h->d_x0, B * 3 * 8)); CKC(cudaMalloc(&h->d_xf, B * 3 * 8)); CKC(cudaMalloc(&h->d_uprev, B * 2 * 8));
-    CKC(cudaMalloc(&h->d_obst, B * MAX_OBST * MPCB200_OBST_STRIDE * 8)); CKC(cudaMalloc(&h->d_obst_count, B * 4));
-    CKC(cudaMalloc(&h->d_obst_type, B * MAX_OBST * 4));
-    h->d_obst_m = MAX_OBST; h->s_obst_m = 0;
-    CKC(cudaMalloc(&h->d_vp, B * MAX_VP * 3 * 8)); CKC(cudaMalloc(&h->d_vp_count, B * 4));
-    CKC(cudaMalloc(&h->d_xinit, B * N * 3 * 8)); CKC(cudaMalloc(&h->d_reinit, B));
-    CKC(cudaMalloc(&h->d_useq, B * N * 2 * 8)); CKC(cudaMalloc(&h->d_xseq, B * N * 3 * 8)); CKC(cudaMalloc(&h->d_dt, B * 8));
-    CKC(cudaMalloc(&h->d_kkt, B * 8)); CKC(cudaMalloc(&h->d_upacked, B * (N - 1) * 2 * 8));
-    CKC(cudaMalloc(&h->d_status, B * 4)); CKC(cudaMalloc(&h->d_iters, B * 4)); CKC(cudaMalloc(&h->d_nactive, 8)); CKC(cudaMalloc(&h->d_queue, 4)); CKC(cudaMalloc(&h->d_smsync, 1024 * 8)); CKC(cudaMalloc(&h->d_prev_iters, B * 4)); CKC(cudaMalloc(&h->d_prev_status, B * 4)); CKC(cudaMalloc(&h->d_order, B * 4));
+    if (io_reserve(h, h->batch, B, 0))
+    {
+        const std::string m = h->err;
+        mpcb200_destroy(h);
+        return set_err(nullptr, MPCB200_E_CUDA, m);
+    }
+    CKC(cudaMalloc(&h->d_nactive, 8)); CKC(cudaMalloc(&h->d_queue, 4)); CKC(cudaMalloc(&h->d_smsync, 1024 * 8)); CKC(cudaMalloc(&h->d_prev_iters, B * 4)); CKC(cudaMalloc(&h->d_prev_status, B * 4)); CKC(cudaMalloc(&h->d_order, B * 4));
     CKC(cudaMalloc(&h->d_origin, 8));
     CKC(cudaMalloc(&h->d_counters, CNT_WORDS * 8)); CKC(cudaMemsetAsync(h->d_counters, 0, CNT_WORDS * 8, h->stream));
-    CKC(allow_smem(phase_kernel<false, MODEL_GENERIC>)); CKC(allow_smem(phase_kernel<true, MODEL_GENERIC>));
-    CKC(allow_smem(phase_kernel<false, MODEL_UNI_POINT>));
     CKC(allow_smem(kkt_warp_kernel<false>)); CKC(allow_smem(kkt_warp_kernel<true>));
-#define ALLOW_FUSED(W_)                                                                                                                  \
-    CKC(allow_smem(solve_fused_kernel<false, false, W_, MODEL_GENERIC>)); CKC(allow_smem(solve_fused_kernel<false, true, W_, MODEL_GENERIC>)); \
-    CKC(allow_smem(solve_fused_kernel<true, false, W_, MODEL_GENERIC>)); CKC(allow_smem(solve_fused_kernel<true, true, W_, MODEL_GENERIC>));   \
-    CKC(allow_smem(solve_fused_kernel<false, false, W_, MODEL_UNI_POINT>)); CKC(allow_smem(solve_fused_kernel<false, true, W_, MODEL_UNI_POINT>))
-    ALLOW_FUSED(SMALL_GROUP_WARPS);
-    ALLOW_FUSED(MAX_GROUP_WARPS);
-#undef ALLOW_FUSED
+    for (const bool lines : {false, true})
+        for (const int model : {MODEL_GENERIC, MODEL_UNI_POINT})
+        {
+            CKC(allow_smem(phase_variant(lines, model)));
+            for (const bool ext : {false, true})
+                for (const bool small : {false, true}) CKC(allow_smem(fused_variant(lines, ext, small, model)));
+        }
     CKC(cudaMallocHost(&h->h_nactive, 8));
-    h->stream_cap = 0;
-    h->s_x0 = h->s_xf = h->s_uprev = h->s_obst = h->s_vp = h->s_useq = h->s_xseq = h->s_dt = h->s_kkt = h->s_upacked = nullptr;
-    h->s_obst_count = h->s_obst_type = h->s_vp_count = h->s_status = h->s_iters = nullptr;
     CKC(cudaEventCreateWithFlags(&h->poll_ev[0], cudaEventDisableTiming)); CKC(cudaEventCreateWithFlags(&h->poll_ev[1], cudaEventDisableTiming));
     CKC(cudaEventCreate(&h->t0)); CKC(cudaEventCreate(&h->t1)); CKC(cudaEventCreate(&h->c0)); CKC(cudaEventCreate(&h->c1));
     int l2_bytes = 0;
@@ -674,18 +730,18 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
 extern "C" void mpcb200_destroy(mpcb200_handle* h)
 {
     if (!h) return;
+    // (also the failure path of mpcb200_create: whatever was not created yet is null)
     cudaSetDevice(h->device);
-    cudaStreamSynchronize(h->stream);
-    void* ptrs[] = {h->ws, h->d_x0, h->d_xf, h->d_uprev, h->d_obst, h->d_obst_count, h->d_obst_type, h->d_vp, h->d_vp_count, h->d_xinit,
-                    h->d_reinit, h->d_useq, h->d_xseq, h->d_dt, h->d_kkt, h->d_upacked, h->d_status, h->d_iters, h->d_nactive, h->d_queue, h->d_flush, h->d_counters, h->d_smsync, h->d_prev_iters, h->d_prev_status, h->d_order, h->d_origin};
+    if (h->stream) cudaStreamSynchronize(h->stream);
+    io_release(h->batch);
+    io_release(h->queue);
+    void* ptrs[] = {h->ws, h->d_nactive, h->d_queue, h->d_flush, h->d_counters, h->d_smsync, h->d_prev_iters, h->d_prev_status, h->d_order,
+                    h->d_origin, h->d_resample, h->d_cm, h->d_fz};
     for (void* p : ptrs) if (p) cudaFree(p);
-    void* sptrs[] = {h->s_x0, h->s_xf, h->s_uprev, h->s_obst, h->s_vp, h->s_useq, h->s_xseq, h->s_dt, h->s_kkt, h->s_upacked, h->s_obst_count,
-                     h->s_obst_type, h->s_vp_count, h->s_status, h->s_iters, h->d_resample, h->d_cm, h->d_fz};
-    for (void* p : sptrs) if (p) cudaFree(p);
     if (h->h_nactive) cudaFreeHost(h->h_nactive);
     for (auto& e : h->ev) cudaEventDestroy(e);
-    cudaEventDestroy(h->poll_ev[0]); cudaEventDestroy(h->poll_ev[1]); cudaEventDestroy(h->t0); cudaEventDestroy(h->t1); cudaEventDestroy(h->c0); cudaEventDestroy(h->c1);
-    cudaStreamDestroy(h->own_stream);
+    for (cudaEvent_t e : {h->poll_ev[0], h->poll_ev[1], h->t0, h->t1, h->c0, h->c1}) if (e) cudaEventDestroy(e);
+    if (h->own_stream) cudaStreamDestroy(h->own_stream);
     delete h;
 }
 
@@ -732,17 +788,21 @@ static int group_threads(const mpcb200_handle* h)
 }
 // robot model / footprint key of the evaluation and line-search code a launch runs (ModelTraits).  The specialised variants exist for
 // the kernels without the rarely used obstacle paths only (LINES = false).
-static int kernel_model(const mpcb200_handle* h)
+static int kernel_model(const mpcb200_handle* h, const IoBuffers& io)
 {
     const bool uni_point = h->cfg.robot_type == MPCB200_ROBOT_UNICYCLE && h->cfg.footprint_type == MPCB200_FOOTPRINT_POINT;
-    return (uni_point && !h->has_lines && !h->force_generic_model) ? MODEL_UNI_POINT : MODEL_GENERIC;
+    return (uni_point && !io.has_lines && !h->force_generic_model) ? MODEL_UNI_POINT : MODEL_GENERIC;
 }
-static int image_words(const mpcb200_handle* h) { return resident_words(h->L, h->has_obst ? (h->obst_max < h->L.M ? h->obst_max : h->L.M) : 0); }
+static int image_words(const mpcb200_handle* h, const InputPtrs& in)
+{
+    return resident_words(h->L, in.obst_count ? (in.obst_max < h->L.M ? in.obst_max : h->L.M) : 0);
+}
 
-static InputPtrs batch_inputs(mpcb200_handle* h, bool with_uprev);
+// one phase kernel over the instance blocks of the batch
 static int launch_phase(mpcb200_handle* h, int phase, int B, int force_cold, int first_outer, int* n_active, bool timed)
 {
-    const int img_words = image_words(h);
+    const IoBuffers& io = h->batch;
+    const int img_words = image_words(h, io.in);
     const size_t img_smem = IMG_HEAD + (size_t)img_words * 8;
     if (img_smem > MAX_IMG_SMEM) return set_err(h, MPCB200_E_UNSUPPORTED, "the instance does not fit in shared memory");
     if (timed && ev_begin(h, phase)) return set_err(h, MPCB200_E_CUDA, "cudaEventCreate failed");
@@ -753,12 +813,10 @@ static int launch_phase(mpcb200_handle* h, int phase, int B, int force_cold, int
     }
     else if (phase >= 0 && phase < MPCB200_NUM_PHASES)
     {
-#define PHASE_DO(LN, MD) phase_kernel<LN, MD><<<B, group_threads(h), img_smem, h->stream>>>(h->cfg, h->L, h->ws, B, phase, h->uprev_dt, force_cold, first_outer, n_active, img_words, batch_inputs(h, true))
-        if (h->has_lines) PHASE_DO(true, MODEL_GENERIC);
-        else if (kernel_model(h) == MODEL_UNI_POINT) PHASE_DO(false, MODEL_UNI_POINT);
-        else PHASE_DO(false, MODEL_GENERIC);
-        h->last_model = kernel_model(h);
-#undef PHASE_DO
+        const int model = kernel_model(h, io);
+        phase_variant(io.has_lines, model)<<<B, group_threads(h), img_smem, h->stream>>>(h->cfg, h->L, h->ws, B, phase, io.uprev_dt, force_cold,
+                                                                                         first_outer, n_active, img_words, io.in);
+        h->last_model = model;
     }
     else return set_err(h, MPCB200_E_INVALID, "unknown phase");
     if (timed) ev_end(h);
@@ -774,130 +832,88 @@ static int check_batch(mpcb200_handle* h, int B)
     return 0;
 }
 
-// which kernel variants a batch needs: line obstacles among the obstacles in use (padding slots are never read)
-static int scan_obstacles(mpcb200_handle* h, size_t B, const mpcb200_obstacles* obst)
+// line obstacles among the obstacles in use (padding slots are never read)
+static bool has_line_obstacles(size_t B, const mpcb200_obstacles* obst)
 {
     const size_t M = (size_t)obst->max_per_instance;
-    int lines = 0;
     for (size_t b = 0; b < B; ++b)
     {
         const int cnt = obst->count[b] < (int)M ? obst->count[b] : (int)M;
-        for (int i = 0; i < cnt; ++i) lines |= obst->type[b * M + i] == MPCB200_OBST_LINE;
+        for (int i = 0; i < cnt; ++i)
+            if (obst->type[b * M + i] == MPCB200_OBST_LINE) return true;
     }
-    h->has_lines = lines || h->cfg.enable_dynamic_obstacles || is_midpoint(h->cfg);
-    return 0;
+    return false;
 }
 
-// host -> device copies of the inputs of `B` instances into the compact staging arrays d (batch) or s (queue job)
-struct Staging { double *x0, *xf, *uprev, *obst, *vp, *xinit; int *obst_count, *obst_type, *vp_count; unsigned char* reinit; };
-static int copy_inputs(mpcb200_handle* h, const Staging& d, size_t B, const double* x0, const double* xf, const double* u_prev, double u_prev_dt,
-                       const mpcb200_obstacles* obst, const mpcb200_viapoints* vp, const double* x_init, const unsigned char* reinit, InputPtrs* in)
+// host -> device copies of the inputs of `B` instances into `io`, and the description of what it now holds (io.in, io.uprev_dt,
+// io.has_lines).  The arguments are checked before anything is copied.
+static int load_inputs(mpcb200_handle* h, IoBuffers& io, int B, const double* x0, const double* xf, const double* u_prev, double u_prev_dt,
+                       const mpcb200_obstacles* obst, const mpcb200_viapoints* vp, const double* x_init, const unsigned char* reinit)
 {
     if (!x0 || !xf) return set_err(h, MPCB200_E_INVALID, "x0 and xf are required");
-    const size_t N = (size_t)h->cfg.n;
-    CK(cudaMemcpyAsync(d.x0, x0, B * 3 * 8, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(d.xf, xf, B * 3 * 8, cudaMemcpyHostToDevice, h->stream));
-    h->stats.h2d_bytes += (long long)(B * 6 * 8);
-    if (u_prev) { CK(cudaMemcpyAsync(d.uprev, u_prev, B * 2 * 8, cudaMemcpyHostToDevice, h->stream)); h->stats.h2d_bytes += (long long)(B * 16); }
-    h->uprev_dt = u_prev_dt;
-    h->has_obst = 0; h->obst_max = 0; h->has_lines = is_midpoint(h->cfg);  // the kernel variants with the rarely used paths compiled in
-    if (obst && obst->count && obst->max_per_instance > 0)
+    const bool with_obst = obst && obst->count && obst->max_per_instance > 0, with_vp = vp && vp->count && vp->max_per_instance > 0;
+    if (with_obst && obst->max_per_instance > MAX_OBST_LIST) return set_err(h, MPCB200_E_UNSUPPORTED, "more than 2048 obstacles per instance");
+    if (with_obst && (!obst->type || !obst->params)) return set_err(h, MPCB200_E_INVALID, "obstacle types and parameters are required");
+    if (with_vp && vp->max_per_instance > MAX_VP) return set_err(h, MPCB200_E_UNSUPPORTED, "more than 8 via-points per instance");
+    if (int rc = io_reserve(h, io, io.rows, with_obst ? obst->max_per_instance : 0)) return rc;
+    const size_t n = (size_t)B, N = (size_t)h->cfg.n;
+    InputPtrs in{io.x0, io.xf, io.uprev, nullptr, io.obst_type, io.obst, 0, nullptr, io.vp, 0, nullptr, nullptr};
+    if (u_prev) { CK(cudaMemcpyAsync(io.uprev, u_prev, n * 2 * 8, cudaMemcpyHostToDevice, h->stream)); h->stats.h2d_bytes += (long long)(n * 16); }
+    else CK(cudaMemsetAsync(io.uprev, 0, n * 2 * 8, h->stream));
+    CK(cudaMemcpyAsync(io.x0, x0, n * 3 * 8, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(io.xf, xf, n * 3 * 8, cudaMemcpyHostToDevice, h->stream));
+    h->stats.h2d_bytes += (long long)(n * 6 * 8);
+    bool lines = is_midpoint(h->cfg);
+    if (with_obst)
     {
-        if (obst->max_per_instance > MAX_OBST_LIST) return set_err(h, MPCB200_E_UNSUPPORTED, "more than 2048 obstacles per instance");
-        if (!obst->type || !obst->params) return set_err(h, MPCB200_E_INVALID, "obstacle types and parameters are required");
         const size_t M = (size_t)obst->max_per_instance;
-        scan_obstacles(h, B, obst);
-        CK(cudaMemcpyAsync(d.obst_count, obst->count, B * 4, cudaMemcpyHostToDevice, h->stream));
-        CK(cudaMemcpyAsync(d.obst_type, obst->type, B * M * 4, cudaMemcpyHostToDevice, h->stream));
-        CK(cudaMemcpyAsync(d.obst, obst->params, B * M * MPCB200_OBST_STRIDE * 8, cudaMemcpyHostToDevice, h->stream));
-        h->stats.h2d_bytes += (long long)(B * 4 + B * M * 4 + B * M * MPCB200_OBST_STRIDE * 8);
-        h->has_obst = 1; h->obst_max = (int)M;
+        CK(cudaMemcpyAsync(io.obst_count, obst->count, n * 4, cudaMemcpyHostToDevice, h->stream));
+        CK(cudaMemcpyAsync(io.obst_type, obst->type, n * M * 4, cudaMemcpyHostToDevice, h->stream));
+        CK(cudaMemcpyAsync(io.obst, obst->params, n * M * MPCB200_OBST_STRIDE * 8, cudaMemcpyHostToDevice, h->stream));
+        h->stats.h2d_bytes += (long long)(n * 4 + n * M * 4 + n * M * MPCB200_OBST_STRIDE * 8);
+        in.obst_count = io.obst_count; in.obst_max = (int)M;
+        lines = lines || h->cfg.enable_dynamic_obstacles || has_line_obstacles(n, obst);
     }
-    h->has_vp = 0; h->vp_max = 0;
-    if (vp && vp->count && vp->max_per_instance > 0)
+    if (with_vp)
     {
-        if (vp->max_per_instance > MAX_VP) return set_err(h, MPCB200_E_UNSUPPORTED, "more than 8 via-points per instance");
         const size_t V = (size_t)vp->max_per_instance;
-        CK(cudaMemcpyAsync(d.vp_count, vp->count, B * 4, cudaMemcpyHostToDevice, h->stream));
-        CK(cudaMemcpyAsync(d.vp, vp->poses, B * V * 3 * 8, cudaMemcpyHostToDevice, h->stream));
-        h->stats.h2d_bytes += (long long)(B * 4 + B * V * 24);
-        h->has_vp = 1; h->vp_max = (int)V;
+        CK(cudaMemcpyAsync(io.vp_count, vp->count, n * 4, cudaMemcpyHostToDevice, h->stream));
+        CK(cudaMemcpyAsync(io.vp, vp->poses, n * V * 3 * 8, cudaMemcpyHostToDevice, h->stream));
+        h->stats.h2d_bytes += (long long)(n * 4 + n * V * 24);
+        in.vp_count = io.vp_count; in.vp_max = (int)V;
     }
-    h->has_xinit = 0;
-    if (x_init && d.xinit) { CK(cudaMemcpyAsync(d.xinit, x_init, B * N * 3 * 8, cudaMemcpyHostToDevice, h->stream)); h->has_xinit = 1; h->stats.h2d_bytes += (long long)(B * N * 24); }
-    h->has_reinit = 0;
-    if (reinit && d.reinit) { CK(cudaMemcpyAsync(d.reinit, reinit, B, cudaMemcpyHostToDevice, h->stream)); h->has_reinit = 1; h->stats.h2d_bytes += (long long)B; }
-    in->x0 = d.x0; in->xf = d.xf; in->u_prev = u_prev ? d.uprev : nullptr;
-    in->obst_count = h->has_obst ? d.obst_count : nullptr; in->obst_type = d.obst_type; in->obst_params = d.obst; in->obst_max = h->obst_max;
-    in->vp_count = h->has_vp ? d.vp_count : nullptr; in->vp_poses = d.vp; in->vp_max = h->vp_max;
-    in->x_init = h->has_xinit ? d.xinit : nullptr;
-    in->reinit = h->has_reinit ? d.reinit : nullptr;
+    if (x_init && io.xinit) { CK(cudaMemcpyAsync(io.xinit, x_init, n * N * 3 * 8, cudaMemcpyHostToDevice, h->stream)); in.x_init = io.xinit; h->stats.h2d_bytes += (long long)(n * N * 24); }
+    if (reinit && io.reinit) { CK(cudaMemcpyAsync(io.reinit, reinit, n, cudaMemcpyHostToDevice, h->stream)); in.reinit = io.reinit; h->stats.h2d_bytes += (long long)n; }
+    io.in = in;
+    io.uprev_dt = u_prev_dt;
+    io.has_lines = lines;
     return 0;
-}
-// obstacle lists longer than the resident list: the staging arrays grow to the list length on first use
-static int reserve_obstacles(mpcb200_handle* h, bool queue, size_t rows, int max_per_instance)
-{
-    if (max_per_instance <= 0 || max_per_instance > MAX_OBST_LIST) return 0;
-    int& cap = queue ? h->s_obst_m : h->d_obst_m;
-    if (max_per_instance <= cap) return 0;
-    double*& par = queue ? h->s_obst : h->d_obst;
-    int*& typ = queue ? h->s_obst_type : h->d_obst_type;
-    CK(cudaStreamSynchronize(h->stream));
-    if (par) cudaFree(par);
-    if (typ) cudaFree(typ);
-    par = nullptr; typ = nullptr; cap = 0;
-    const size_t M = (size_t)max_per_instance;
-    CK(cudaMalloc(&par, rows * M * MPCB200_OBST_STRIDE * 8));
-    CK(cudaMalloc(&typ, rows * M * 4));
-    cap = (int)M;
-    return 0;
-}
-static Staging batch_staging(mpcb200_handle* h) { return Staging{h->d_x0, h->d_xf, h->d_uprev, h->d_obst, h->d_vp, h->d_xinit, h->d_obst_count, h->d_obst_type, h->d_vp_count, h->d_reinit}; }
-static InputPtrs batch_inputs(mpcb200_handle* h, bool with_uprev)
-{
-    InputPtrs in;
-    in.x0 = h->d_x0; in.xf = h->d_xf; in.u_prev = with_uprev ? h->d_uprev : nullptr;
-    in.obst_count = h->has_obst ? h->d_obst_count : nullptr; in.obst_type = h->d_obst_type; in.obst_params = h->d_obst; in.obst_max = h->obst_max;
-    in.vp_count = h->has_vp ? h->d_vp_count : nullptr; in.vp_poses = h->d_vp; in.vp_max = h->vp_max;
-    in.x_init = h->has_xinit ? h->d_xinit : nullptr;
-    in.reinit = h->has_reinit ? h->d_reinit : nullptr;
-    return in;
 }
 
-static int upload_inputs(mpcb200_handle* h, int B, const double* x0, const double* xf, const double* u_prev, double u_prev_dt,
-                         const mpcb200_obstacles* obst, const mpcb200_viapoints* vp, const double* x_init, const unsigned char* reinit)
+// the batch's inputs into the instance blocks as well: the kernel-level API and the phased solve work on the blocks
+static int scatter_to_blocks(mpcb200_handle* h, int B)
 {
-    CK(cudaSetDevice(h->device));
-    InputPtrs in;
-    if (!u_prev) CK(cudaMemsetAsync(h->d_uprev, 0, (size_t)B * 2 * 8, h->stream));
-    int rc = reserve_obstacles(h, false, (size_t)h->max_batch, (obst && obst->count) ? obst->max_per_instance : 0);
-    if (rc) return rc;
-    rc = copy_inputs(h, batch_staging(h), (size_t)B, x0, xf, u_prev, u_prev_dt, obst, vp, x_init, reinit, &in);
-    if (rc) return rc;
-    // the instance blocks get the inputs as well: the kernel-level API (phase kernels) works on the blocks
-    in.u_prev = h->d_uprev;
-    scatter_inputs_kernel<<<grid_for(B, WARPS_PER_CTA), WARPS_PER_CTA * 32, 0, h->stream>>>(h->L, h->ws, B, in);
+    scatter_inputs_kernel<<<grid_for(B, WARPS_PER_CTA), WARPS_PER_CTA * 32, 0, h->stream>>>(h->L, h->ws, B, h->batch.in);
     h->stats.launches_total += 1;
     CK(cudaGetLastError());
-    h->B = B;
     return 0;
 }
 
 // ---- the solve: one launch of the persistent kernel over a queue of `total` instances ----
-static int launch_fused(mpcb200_handle* h, int total, int queue_mode, int force_cold, const InputPtrs& in, const OutputPtrs& out)
+static int launch_fused(mpcb200_handle* h, const IoBuffers& io, int total, int queue_mode, int force_cold)
 {
     FusedArgs a;
-    a.ws = h->ws; a.in = in; a.out = out; a.total = total; a.queue_mode = queue_mode; a.force_cold = force_cold; a.uprev_dt = h->uprev_dt;
-    a.img_words = image_words(h); a.queue = h->d_queue; a.counters = h->d_counters;
+    a.ws = h->ws; a.in = io.in; a.out = io.out(); a.total = total; a.queue_mode = queue_mode; a.force_cold = force_cold; a.uprev_dt = io.uprev_dt;
+    a.img_words = image_words(h, io.in); a.queue = h->d_queue; a.counters = h->d_counters;
     a.sm_sync = nullptr; a.sm_gates = h->sm_phase_sync == 2 ? 2 : 3;
     a.order = nullptr;
     a.budget_ns = h->budget_ns; a.origin = h->d_origin;
     if (h->budget_ns) CK(cudaMemsetAsync(h->d_origin, 0, 8, h->stream));
     if (!queue_mode && h->order_by_history && h->hist_B == total && total > h->num_sms)
     {
-        // (d_iters and d_status are rewritten by this solve: order from copies)
-        CK(cudaMemcpyAsync(h->d_prev_iters, h->d_iters, (size_t)total * 4, cudaMemcpyDeviceToDevice, h->stream));
-        CK(cudaMemcpyAsync(h->d_prev_status, h->d_status, (size_t)total * 4, cudaMemcpyDeviceToDevice, h->stream));
+        // (the iteration counts and statuses are rewritten by this solve: order from copies)
+        CK(cudaMemcpyAsync(h->d_prev_iters, io.iters, (size_t)total * 4, cudaMemcpyDeviceToDevice, h->stream));
+        CK(cudaMemcpyAsync(h->d_prev_status, io.status, (size_t)total * 4, cudaMemcpyDeviceToDevice, h->stream));
         order_by_history_kernel<<<1, 1024, 0, h->stream>>>(h->d_prev_iters, h->d_prev_status, h->cfg.max_iter, total, h->d_order);
         h->stats.launches_total += 1;
         a.order = h->d_order;
@@ -905,32 +921,23 @@ static int launch_fused(mpcb200_handle* h, int total, int queue_mode, int force_
     if (!queue_mode) h->hist_B = total;
     const size_t smem = IMG_HEAD + (size_t)a.img_words * 8;
     if (smem > MAX_IMG_SMEM) return set_err(h, MPCB200_E_UNSUPPORTED, "the instance does not fit in shared memory");
-    const int threads = group_threads(h);
-    const bool ext = kkt_is_ext(h->cfg), small = threads <= SMALL_GROUP_WARPS * 32;
+    const int threads = group_threads(h), model = kernel_model(h, io);
+    const FusedKernel kernel = fused_variant(io.has_lines, kkt_is_ext(h->cfg), threads <= SMALL_GROUP_WARPS * 32, model);
     int per_sm = 0;
-#define FUSED_DO(LN, EX, MD) do { if (small) FUSED_SHAPE(LN, EX, SMALL_GROUP_WARPS, MD); else FUSED_SHAPE(LN, EX, MAX_GROUP_WARPS, MD); } while (0)
-#define FUSED_SHAPE(LN, EX, WS, MD)                                                                                            \
-    do {                                                                                                                       \
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, solve_fused_kernel<LN, EX, WS, MD>, threads, smem));         \
-        if (per_sm < 1) return set_err(h, MPCB200_E_UNSUPPORTED, "the solve kernel does not fit on an SM with this configuration"); \
-        if (h->max_ctas_per_sm > 0 && per_sm > h->max_ctas_per_sm) per_sm = h->max_ctas_per_sm;                                \
-        const int grid = total < per_sm * h->num_sms ? total : per_sm * h->num_sms;                                            \
-        h->fused_grid = grid;                                                                                                  \
-        /* phase alignment pays when several CTAs share an SM (auto: from three CTAs per SM) */                                 \
-        if (h->sm_phase_sync > 0 || (h->sm_phase_sync < 0 && per_sm >= 3 && grid > h->num_sms))                                \
-        {                                                                                                                      \
-            a.sm_sync = h->d_smsync;                                                                                           \
-            CK(cudaMemsetAsync(h->d_smsync, 0, 1024 * 8, h->stream));                                                          \
-        }                                                                                                                      \
-        CK(cudaMemsetAsync(h->d_queue, 0, 4, h->stream));                                                                      \
-        solve_fused_kernel<LN, EX, WS, MD><<<grid, threads, smem, h->stream>>>(h->cfg, h->L, a);                               \
-    } while (0)
-    if (h->has_lines) { if (ext) FUSED_DO(true, true, MODEL_GENERIC); else FUSED_DO(true, false, MODEL_GENERIC); }
-    else if (kernel_model(h) == MODEL_UNI_POINT) { if (ext) FUSED_DO(false, true, MODEL_UNI_POINT); else FUSED_DO(false, false, MODEL_UNI_POINT); }
-    else { if (ext) FUSED_DO(false, true, MODEL_GENERIC); else FUSED_DO(false, false, MODEL_GENERIC); }
-    h->last_model = kernel_model(h);
-#undef FUSED_SHAPE
-#undef FUSED_DO
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
+    if (per_sm < 1) return set_err(h, MPCB200_E_UNSUPPORTED, "the solve kernel does not fit on an SM with this configuration");
+    if (h->max_ctas_per_sm > 0 && per_sm > h->max_ctas_per_sm) per_sm = h->max_ctas_per_sm;
+    const int grid = total < per_sm * h->num_sms ? total : per_sm * h->num_sms;
+    h->fused_grid = grid;
+    // phase alignment pays when several CTAs share an SM (auto: from three CTAs per SM)
+    if (h->sm_phase_sync > 0 || (h->sm_phase_sync < 0 && per_sm >= 3 && grid > h->num_sms))
+    {
+        a.sm_sync = h->d_smsync;
+        CK(cudaMemsetAsync(h->d_smsync, 0, 1024 * 8, h->stream));
+    }
+    CK(cudaMemsetAsync(h->d_queue, 0, 4, h->stream));
+    kernel<<<grid, threads, smem, h->stream>>>(h->cfg, h->L, a);
+    h->last_model = model;
     h->stats.launches_total += 1;
     CK(cudaGetLastError());
     return 0;
@@ -974,8 +981,7 @@ static int solve_phased(mpcb200_handle* h, int B, int force_cold)
             if ((rc = launch_phase(h, MPCB200_PHASE_LINESEARCH, B, 0, 0, nullptr, timed(MPCB200_PHASE_LINESEARCH)))) return rc;
         }
     }
-    OutputPtrs o{h->d_useq, h->d_xseq, h->d_dt, h->d_status, h->d_kkt, h->d_iters, h->d_upacked};
-    gather_outputs_kernel<<<grid_for(B, WARPS_PER_CTA), WARPS_PER_CTA * 32, 0, h->stream>>>(h->L, h->ws, B, o);
+    gather_outputs_kernel<<<grid_for(B, WARPS_PER_CTA), WARPS_PER_CTA * 32, 0, h->stream>>>(h->L, h->ws, B, h->batch.out());
     h->stats.launches_total += 1;
     CK(cudaGetLastError());
     return 0;
@@ -1005,16 +1011,12 @@ static int check_budget_mode(mpcb200_handle* h)
     return 0;
 }
 
-static int solve_device(mpcb200_handle* h, int B, int force_cold, double* solve_time_s)
+// One solve between the events t0 and t1: the batch (fused or phased, by the solve mode) or the queue job (always fused).
+// Reports the device time of the solve and folds the counters of the fused kernel into the statistics.
+static int timed_launch(mpcb200_handle* h, const IoBuffers& io, int total, int queue_mode, int force_cold, double* solve_time_s)
 {
     CK(cudaEventRecord(h->t0, h->stream));
-    int rc;
-    if (h->solve_mode == 1) rc = solve_phased(h, B, force_cold);
-    else
-    {
-        OutputPtrs o{h->d_useq, h->d_xseq, h->d_dt, h->d_status, h->d_kkt, h->d_iters, h->d_upacked};
-        rc = launch_fused(h, B, 0, force_cold, batch_inputs(h, true), o);
-    }
+    const int rc = (h->solve_mode == 1 && !queue_mode) ? solve_phased(h, total, force_cold) : launch_fused(h, io, total, queue_mode, force_cold);
     if (rc) return rc;
     CK(cudaEventRecord(h->t1, h->stream));
     CK(cudaStreamSynchronize(h->stream));
@@ -1025,38 +1027,21 @@ static int solve_device(mpcb200_handle* h, int B, int force_cold, double* solve_
     return collect_fused_counters(h);
 }
 
-static int fetch_results(mpcb200_handle* h, int B, double* u_seq, double* x_seq, double* dt_out, int* status, double* kkt_err, int* iters)
+// results of `B` instances from `io` to the host (a null destination is skipped)
+static int fetch_outputs(mpcb200_handle* h, const IoBuffers& io, int B, double* u_seq, double* x_seq, double* dt_out, int* status, double* kkt_err, int* iters)
 {
-    const size_t N = (size_t)h->cfg.n;
-    if (u_seq) { CK(cudaMemcpyAsync(u_seq, h->d_useq, (size_t)B * N * 16, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(B * N * 16); }
-    if (x_seq) { CK(cudaMemcpyAsync(x_seq, h->d_xseq, (size_t)B * N * 24, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(B * N * 24); }
-    if (dt_out) { CK(cudaMemcpyAsync(dt_out, h->d_dt, (size_t)B * 8, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += B * 8; }
-    if (status) { CK(cudaMemcpyAsync(status, h->d_status, (size_t)B * 4, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += B * 4; }
-    if (kkt_err) { CK(cudaMemcpyAsync(kkt_err, h->d_kkt, (size_t)B * 8, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += B * 8; }
-    if (iters) { CK(cudaMemcpyAsync(iters, h->d_iters, (size_t)B * 4, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += B * 4; }
+    const size_t n = (size_t)B, N = (size_t)h->cfg.n;
+    if (u_seq) { CK(cudaMemcpyAsync(u_seq, io.useq, n * N * 16, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(n * N * 16); }
+    if (x_seq) { CK(cudaMemcpyAsync(x_seq, io.xseq, n * N * 24, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(n * N * 24); }
+    if (dt_out) { CK(cudaMemcpyAsync(dt_out, io.dt, n * 8, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(n * 8); }
+    if (status) { CK(cudaMemcpyAsync(status, io.status, n * 4, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(n * 4); }
+    if (kkt_err) { CK(cudaMemcpyAsync(kkt_err, io.kkt, n * 8, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(n * 8); }
+    if (iters) { CK(cudaMemcpyAsync(iters, io.iters, n * 4, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(n * 4); }
     CK(cudaStreamSynchronize(h->stream));
     return 0;
 }
 
 // ---- queue solve: `total` cold instances through the persistent kernel (continuous batching) ----------------------
-static int stream_reserve(mpcb200_handle* h, size_t total)
-{
-    if (total <= h->stream_cap) return 0;
-    void* old[] = {h->s_x0, h->s_xf, h->s_uprev, h->s_obst, h->s_vp, h->s_useq, h->s_xseq, h->s_dt, h->s_kkt, h->s_upacked, h->s_obst_count,
-                   h->s_obst_type, h->s_vp_count, h->s_status, h->s_iters};
-    for (void* p : old) if (p) cudaFree(p);
-    h->stream_cap = 0; h->s_obst_m = 0;
-    const size_t N = (size_t)h->n_cap, T = total;  // sized for the largest horizon the handle can be resampled to
-    CK(cudaMalloc(&h->s_x0, T * 3 * 8)); CK(cudaMalloc(&h->s_xf, T * 3 * 8)); CK(cudaMalloc(&h->s_uprev, T * 2 * 8));
-    CK(cudaMalloc(&h->s_obst, T * MAX_OBST * MPCB200_OBST_STRIDE * 8)); CK(cudaMalloc(&h->s_obst_count, T * 4)); CK(cudaMalloc(&h->s_obst_type, T * MAX_OBST * 4));
-    h->s_obst_m = MAX_OBST;
-    CK(cudaMalloc(&h->s_vp, T * MAX_VP * 3 * 8)); CK(cudaMalloc(&h->s_vp_count, T * 4));
-    CK(cudaMalloc(&h->s_useq, T * N * 2 * 8)); CK(cudaMalloc(&h->s_xseq, T * N * 3 * 8)); CK(cudaMalloc(&h->s_dt, T * 8)); CK(cudaMalloc(&h->s_kkt, T * 8));
-    CK(cudaMalloc(&h->s_upacked, T * (N - 1) * 2 * 8)); CK(cudaMalloc(&h->s_status, T * 4)); CK(cudaMalloc(&h->s_iters, T * 4));
-    h->stream_cap = total;
-    return 0;
-}
-
 extern "C" int mpcb200_solve_stream(mpcb200_handle* h, int total, const double* x0, const double* xf, const double* u_prev, double u_prev_dt,
                                     const mpcb200_obstacles* obst, const mpcb200_viapoints* vp, double* u_seq, double* x_seq, double* dt_out,
                                     int* status, double* kkt_err, int* iters, double* solve_time_s)
@@ -1064,31 +1049,11 @@ extern "C" int mpcb200_solve_stream(mpcb200_handle* h, int total, const double* 
     if (!h) return MPCB200_E_INVALID;
     if (total < 1 || !x0 || !xf) return set_err(h, MPCB200_E_INVALID, "total >= 1, x0 and xf are required");
     CK(cudaSetDevice(h->device));
-    int rc = stream_reserve(h, (size_t)total);
-    if (rc) return rc;
-    if ((rc = reserve_obstacles(h, true, h->stream_cap, (obst && obst->count) ? obst->max_per_instance : 0))) return rc;
-    const size_t T = (size_t)total, N = (size_t)h->cfg.n;
-    InputPtrs in;
-    Staging s{h->s_x0, h->s_xf, h->s_uprev, h->s_obst, h->s_vp, nullptr, h->s_obst_count, h->s_obst_type, h->s_vp_count, nullptr};
-    if ((rc = copy_inputs(h, s, T, x0, xf, u_prev, u_prev_dt, obst, vp, nullptr, nullptr, &in))) return rc;
-    OutputPtrs o{h->s_useq, h->s_xseq, h->s_dt, h->s_status, h->s_kkt, h->s_iters, h->s_upacked};
-    CK(cudaEventRecord(h->t0, h->stream));
-    if ((rc = launch_fused(h, total, 1, 1, in, o))) return rc;
-    CK(cudaEventRecord(h->t1, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    float ms = 0.f;
-    CK(cudaEventElapsedTime(&ms, h->t0, h->t1));
-    if (solve_time_s) *solve_time_s = ms * 1e-3;
-    if ((rc = collect_fused_counters(h))) return rc;
-    // ---- results of the whole job ----
-    if (u_seq) { CK(cudaMemcpyAsync(u_seq, h->s_useq, T * N * 16, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(T * N * 16); }
-    if (x_seq) { CK(cudaMemcpyAsync(x_seq, h->s_xseq, T * N * 24, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(T * N * 24); }
-    if (dt_out) { CK(cudaMemcpyAsync(dt_out, h->s_dt, T * 8, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(T * 8); }
-    if (status) { CK(cudaMemcpyAsync(status, h->s_status, T * 4, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(T * 4); }
-    if (kkt_err) { CK(cudaMemcpyAsync(kkt_err, h->s_kkt, T * 8, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(T * 8); }
-    if (iters) { CK(cudaMemcpyAsync(iters, h->s_iters, T * 4, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(T * 4); }
-    CK(cudaStreamSynchronize(h->stream));
-    return 0;
+    int rc;
+    if ((rc = io_reserve(h, h->queue, (size_t)total, 0))) return rc;
+    if ((rc = load_inputs(h, h->queue, total, x0, xf, u_prev, u_prev_dt, obst, vp, nullptr, nullptr))) return rc;
+    if ((rc = timed_launch(h, h->queue, total, 1, 1, solve_time_s))) return rc;
+    return fetch_outputs(h, h->queue, total, u_seq, x_seq, dt_out, status, kkt_err, iters);
 }
 
 extern "C" int mpcb200_step_batch(mpcb200_handle* h, int B, const double* x0, const double* xf, const double* u_prev, double u_prev_dt,
@@ -1100,21 +1065,12 @@ extern "C" int mpcb200_step_batch(mpcb200_handle* h, int B, const double* x0, co
     if (rc) return rc;
     if ((rc = check_budget_mode(h))) return rc;
     CK(cudaSetDevice(h->device));
-    if (h->solve_mode == 1)
-    {
-        if ((rc = upload_inputs(h, B, x0, xf, u_prev, u_prev_dt, obst, vp, x_init, reinit))) return rc;
-    }
-    else
-    {
-        // fused mode: the solve kernel reads the compact arrays itself, the blocks only carry the warm state
-        InputPtrs in;
-        if (!u_prev) CK(cudaMemsetAsync(h->d_uprev, 0, (size_t)B * 2 * 8, h->stream));
-        if ((rc = reserve_obstacles(h, false, (size_t)h->max_batch, (obst && obst->count) ? obst->max_per_instance : 0))) return rc;
-        if ((rc = copy_inputs(h, batch_staging(h), (size_t)B, x0, xf, u_prev, u_prev_dt, obst, vp, x_init, reinit, &in))) return rc;
-        h->B = B;
-    }
-    if ((rc = solve_device(h, B, 0, solve_time_s))) return rc;
-    return fetch_results(h, B, u_seq, x_seq, dt_out, status, kkt_err, iters);
+    if ((rc = load_inputs(h, h->batch, B, x0, xf, u_prev, u_prev_dt, obst, vp, x_init, reinit))) return rc;
+    // the phased mode works on the instance blocks; the fused kernel reads the compact arrays itself
+    if (h->solve_mode == 1 && (rc = scatter_to_blocks(h, B))) return rc;
+    h->B = B;
+    if ((rc = timed_launch(h, h->batch, B, 0, 0, solve_time_s))) return rc;
+    return fetch_outputs(h, h->batch, B, u_seq, x_seq, dt_out, status, kkt_err, iters);
 }
 
 extern "C" int mpcb200_upload_inputs(mpcb200_handle* h, int B, const double* x0, const double* xf, const double* u_prev, double u_prev_dt,
@@ -1122,7 +1078,10 @@ extern "C" int mpcb200_upload_inputs(mpcb200_handle* h, int B, const double* x0,
 {
     int rc = check_batch(h, B);
     if (rc) return rc;
-    if ((rc = upload_inputs(h, B, x0, xf, u_prev, u_prev_dt, obst, vp, x_init, nullptr))) return rc;
+    CK(cudaSetDevice(h->device));
+    if ((rc = load_inputs(h, h->batch, B, x0, xf, u_prev, u_prev_dt, obst, vp, x_init, nullptr))) return rc;
+    if ((rc = scatter_to_blocks(h, B))) return rc;
+    h->B = B;
     CK(cudaStreamSynchronize(h->stream));
     return 0;
 }
@@ -1132,20 +1091,20 @@ extern "C" int mpcb200_solve_resident(mpcb200_handle* h, int cold, double* solve
     if (!h || h->B < 1) return set_err(h, MPCB200_E_INVALID, "no resident inputs: call mpcb200_upload_inputs first");
     if (int rc = check_budget_mode(h)) return rc;
     CK(cudaSetDevice(h->device));
-    return solve_device(h, h->B, cold ? 1 : 0, solve_time_s);
+    return timed_launch(h, h->batch, h->B, 0, cold ? 1 : 0, solve_time_s);
 }
 
 extern "C" int mpcb200_fetch_results(mpcb200_handle* h, double* u_seq, double* x_seq, double* dt_out, int* status, double* kkt_err, int* iters)
 {
     if (!h || h->B < 1) return set_err(h, MPCB200_E_INVALID, "nothing to fetch");
     CK(cudaSetDevice(h->device));
-    return fetch_results(h, h->B, u_seq, x_seq, dt_out, status, kkt_err, iters);
+    return fetch_outputs(h, h->batch, h->B, u_seq, x_seq, dt_out, status, kkt_err, iters);
 }
 
 extern "C" int mpcb200_device_controls(mpcb200_handle* h, void** dev_ptr, long long* n_doubles)
 {
     if (!h || h->B < 1) return set_err(h, MPCB200_E_INVALID, "no batch solved yet");
-    if (dev_ptr) *dev_ptr = h->d_upacked;
+    if (dev_ptr) *dev_ptr = h->batch.upacked;
     if (n_doubles) *n_doubles = (long long)h->B * (h->cfg.n - 1) * 2;
     return 0;
 }
@@ -1156,8 +1115,8 @@ extern "C" int mpcb200_reset(mpcb200_handle* h, const unsigned char* which, int 
     CK(cudaSetDevice(h->device));
     const int n = which ? B : h->max_batch;
     if (n < 1 || n > h->max_batch) return set_err(h, MPCB200_E_INVALID, "batch size out of range");
-    if (which) CK(cudaMemcpyAsync(h->d_reinit, which, (size_t)n, cudaMemcpyHostToDevice, h->stream));
-    reset_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(h->L, h->ws, n, which ? h->d_reinit : nullptr);
+    if (which) CK(cudaMemcpyAsync(h->batch.reinit, which, (size_t)n, cudaMemcpyHostToDevice, h->stream));
+    reset_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(h->L, h->ws, n, which ? h->batch.reinit : nullptr);
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(h->stream));
     return 0;
@@ -1368,7 +1327,7 @@ extern "C" int mpcb200_export_controls(mpcb200_handle* h, void* dst_dev)
 {
     if (!h || h->B < 1 || !dst_dev) return set_err(h, MPCB200_E_INVALID, "nothing to export");
     CK(cudaSetDevice(h->device));
-    CK(cudaMemcpyAsync(dst_dev, h->d_upacked, (size_t)h->B * (h->cfg.n - 1) * 16, cudaMemcpyDeviceToDevice, h->stream));
+    CK(cudaMemcpyAsync(dst_dev, h->batch.upacked, (size_t)h->B * (h->cfg.n - 1) * 16, cudaMemcpyDeviceToDevice, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return 0;
 }
@@ -1466,25 +1425,18 @@ extern "C" int mpcb200_step_batch_costmap(mpcb200_handle* h, int B, const double
     if (max_per_instance < 1 || max_per_instance > MAX_OBST_LIST) return set_err(h, MPCB200_E_UNSUPPORTED, "step_batch_costmap: 1..2048 obstacles per instance");
     if ((rc = check_budget_mode(h))) return rc;
     CK(cudaSetDevice(h->device));
+    IoBuffers& io = h->batch;
     // room for the lists in the batch's obstacle arrays
-    if ((rc = reserve_obstacles(h, false, (size_t)h->max_batch, max_per_instance))) return rc;
-    InputPtrs in;
-    if (!u_prev) CK(cudaMemsetAsync(h->d_uprev, 0, (size_t)B * 2 * 8, h->stream));
-    if ((rc = copy_inputs(h, batch_staging(h), (size_t)B, x0, xf, u_prev, u_prev_dt, nullptr, vp, x_init, reinit, &in))) return rc;
+    if ((rc = io_reserve(h, io, io.rows, max_per_instance))) return rc;
+    if ((rc = load_inputs(h, io, B, x0, xf, u_prev, u_prev_dt, nullptr, vp, x_init, reinit))) return rc;
     CostmapOut o;
-    if ((rc = costmap_run(h, B, maps, nullptr, h->d_x0, behind_robot_dist, max_per_instance, h->d_obst_count, h->d_obst_type, h->d_obst, &o))) return rc;
-    h->has_obst = 1; h->obst_max = max_per_instance;   // point obstacles only: no line-obstacle kernel variant needed
+    if ((rc = costmap_run(h, B, maps, nullptr, io.x0, behind_robot_dist, max_per_instance, io.obst_count, io.obst_type, io.obst, &o))) return rc;
+    io.in.obst_count = io.obst_count; io.in.obst_max = max_per_instance;   // point obstacles only: no line-obstacle kernel variant needed
     h->B = B;
-    if (h->solve_mode == 1)
-    {
-        in = batch_inputs(h, true);
-        scatter_inputs_kernel<<<grid_for(B, WARPS_PER_CTA), WARPS_PER_CTA * 32, 0, h->stream>>>(h->L, h->ws, B, in);
-        h->stats.launches_total += 1;
-        CK(cudaGetLastError());
-    }
-    if ((rc = solve_device(h, B, 0, solve_time_s))) return rc;
+    if (h->solve_mode == 1 && (rc = scatter_to_blocks(h, B))) return rc;
+    if ((rc = timed_launch(h, io, B, 0, 0, solve_time_s))) return rc;
     if (obst_found) CK(cudaMemcpyAsync(obst_found, o.found, (size_t)B * 4, cudaMemcpyDeviceToHost, h->stream));
-    rc = fetch_results(h, B, u_seq, x_seq, dt_out, status, kkt_err, iters);
+    rc = fetch_outputs(h, io, B, u_seq, x_seq, dt_out, status, kkt_err, iters);
     float ms = 0.f;
     if (!rc && cudaEventElapsedTime(&ms, h->c0, h->c1) == cudaSuccess) h->costmap_ms = ms;
     return rc;
@@ -1524,7 +1476,7 @@ extern "C" int mpcb200_check_feasible(mpcb200_handle* h, int B, const mpcb200_co
     if (n_footprint > 0) CK(cudaMemcpyAsync(d_fp, footprint_xy, (size_t)n_footprint * 16, cudaMemcpyHostToDevice, h->stream));
     if (x_seq) CK(cudaMemcpyAsync(d_x, x_seq, (size_t)B * n * 24, cudaMemcpyHostToDevice, h->stream));
     h->stats.h2d_bytes += (long long)((size_t)B * W * H + (size_t)B * 16 + (size_t)n_footprint * 16 + (x_seq ? (size_t)B * n * 24 : 0));
-    FeasArgs a{maps->size_x, maps->size_y, maps->resolution, d_cost, d_origin, x_seq ? d_x : h->d_xseq, n, d_fp, n_footprint,
+    FeasArgs a{maps->size_x, maps->size_y, maps->resolution, d_cost, d_origin, x_seq ? d_x : h->batch.xseq, n, d_fp, n_footprint,
                inscribed_radius, min_resolution_angular, look_ahead_idx};
     feasible_kernel<<<grid_for(B, WARPS_PER_CTA), WARPS_PER_CTA * 32, 0, h->stream>>>(a, B, d_ok);
     h->stats.launches_total += 1;
@@ -1698,7 +1650,7 @@ extern "C" int mpcb200_step_batch_multi(mpcb200_multi* m, int B, const double* x
         for (int r = 0; r < G && nrc == 0; ++r)
         {
             cudaSetDevice(m->devices[r]);
-            nrc = m->nccl.AllGather(m->h[r]->d_upacked, m->d_all[r], count, MPC_NCCL_FLOAT64, m->comm[r], m->h[r]->stream);
+            nrc = m->nccl.AllGather(m->h[r]->batch.upacked, m->d_all[r], count, MPC_NCCL_FLOAT64, m->comm[r], m->h[r]->stream);
         }
         const int erc = m->nccl.GroupEnd();
         if (nrc == 0) nrc = erc;
@@ -1712,7 +1664,7 @@ extern "C" int mpcb200_step_batch_multi(mpcb200_multi* m, int B, const double* x
     else
     {
         cudaSetDevice(m->devices[0]);
-        if (cudaMemcpyAsync(m->d_all[0], m->h[0]->d_upacked, count * 8, cudaMemcpyDeviceToDevice, m->h[0]->stream) != cudaSuccess ||
+        if (cudaMemcpyAsync(m->d_all[0], m->h[0]->batch.upacked, count * 8, cudaMemcpyDeviceToDevice, m->h[0]->stream) != cudaSuccess ||
             cudaStreamSynchronize(m->h[0]->stream) != cudaSuccess)
             return multi_err(m, MPCB200_E_CUDA, "copy of the controls failed");
     }

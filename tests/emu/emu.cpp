@@ -277,7 +277,7 @@ void emu_linesearch(const Cfg* cp, double* W, double uprev_dt)
     if (tiny >= (double)TINY_STEP_COUNT) ASC(MPCB200_SC_STATUS) = (double)MPCB200_STATUS_NUMERICAL_ERROR;  /* jammed: give up */
 }
 
-// whole Controller::step of one instance, same launch sequence as solve_device() in mpcb200.cu
+// whole Controller::step of one instance, same launch sequence as solve_phased() in mpcb200.cu
 int emu_solve(const Cfg* cp, double* W, double uprev_dt, int force_cold)
 {
     const Cfg& c = *cp;

@@ -380,3 +380,22 @@ def test_execution_options_do_not_change_results(cuda_lib):
     # with the history the second solve starts its longest instances first: it must not be clearly slower than index order
     # (loose bound: a timing, not a result)
     assert times[(-1, 0, 1)] <= 1.3 * times[(-1, 0, 0)]
+
+
+def test_queue_job_leaves_resident_batch_alone(cuda_lib):
+    """The batch and the queue job have inputs of their own: a queue solve without obstacles and with another u_prev_dt
+    between two cold solves of the resident batch does not change what the resident batch is solved with."""
+    cfg = configs.cfg2(tol=1e-6)
+    B = 64
+    data = configs.generate(2, B)
+    other = configs.generate(2, B, first=B)
+    s = capi.BatchSolver(cfg, B, device=0)
+    s.upload(data["x0"], data["xf"], data["u_prev"], data["u_prev_dt"], data["obstacles"], None)
+    s.solve_resident(cold=True)
+    r1 = s.fetch()
+    s.solve_stream(other["x0"], other["xf"], other["u_prev"], other["u_prev_dt"] + 0.1, None, None)
+    s.solve_resident(cold=True)
+    r2 = s.fetch()
+    s.close()
+    for k in ("status", "iters", "u_seq", "x_seq", "dt", "kkt_err"):
+        np.testing.assert_array_equal(r2[k], r1[k], err_msg=k)
