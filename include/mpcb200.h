@@ -437,8 +437,9 @@ int mpcb200_set_stream(mpcb200_handle* h, void* cuda_stream);
    cycle tends to be hard in this one).  Order of execution only; 0 = index order. */
 #define MPCB200_OPT_ORDER_BY_HISTORY 6
 /* MPCB200_OPT_FORCE_GENERIC_MODEL: 0 (default) = a unicycle with a point footprint (and no line or moving obstacles, no midpoint
-   differences) runs solve kernels compiled for that model: the robot and footprint tests fold at compile time; 1 = always the
-   kernels that read the model from the configuration.  Both compute the same results bit for bit (A/B comparisons). */
+   differences) runs solve kernels compiled for that model: the robot and footprint tests fold at compile time, and for the
+   fixed-dt quadratic form (MPCB200_PROBLEM_FIXED_DT_QF) the tests of the problem fields too; 1 = always the kernels that read the
+   model and the problem from the configuration.  Both compute the same results bit for bit (A/B comparisons). */
 #define MPCB200_OPT_FORCE_GENERIC_MODEL 7
 int mpcb200_set_option(mpcb200_handle* h, int option, int value);
 /* Model key of the evaluation / line-search code of the last solve launch of this handle: MPCB200_MODEL_GENERIC (also before the
@@ -446,6 +447,13 @@ int mpcb200_set_option(mpcb200_handle* h, int option, int value);
 #define MPCB200_MODEL_GENERIC 0
 #define MPCB200_MODEL_UNI_POINT 1
 int mpcb200_kernel_model(const mpcb200_handle* h);
+/* Problem key of the same code: MPCB200_PROBLEM_GENERIC (read from the configuration; also before the first solve) or
+   MPCB200_PROBLEM_FIXED_DT_QF (compiled for the fixed-dt quadratic form: no integral form or minimum-time term, no terminal ball, no
+   fixed final state component, finite u_lb / u_ub / du_lb / du_ub on both controls).  The fixed-dt key exists with the unicycle /
+   point-footprint model key only (MPCB200_OPT_FORCE_GENERIC_MODEL turns both off). */
+#define MPCB200_PROBLEM_GENERIC 0
+#define MPCB200_PROBLEM_FIXED_DT_QF 1
+int mpcb200_kernel_problem(const mpcb200_handle* h);
 
 /* Counters accumulated since the last mpcb200_stats_reset: kernels launched, device ms per phase. */
 typedef struct mpcb200_stats {

@@ -35,6 +35,7 @@ OPT_SM_PHASE_SYNC = 5
 OPT_ORDER_BY_HISTORY = 6
 OPT_FORCE_GENERIC_MODEL = 7
 MODEL_GENERIC, MODEL_UNI_POINT = 0, 1
+PROBLEM_GENERIC, PROBLEM_FIXED_DT_QF = 0, 1
 SOLVE_FUSED, SOLVE_PHASED = 0, 1
 NUM_PHASES = 5
 K_H, K_G, K_A, K_B, K_E, K_C, K_HB, K_D = 0, 15, 20, 23, 29, 32, 34, 39
@@ -199,7 +200,7 @@ EXPORTS = [
     "mpcb200_default_config", "mpcb200_create", "mpcb200_step_batch", "mpcb200_reset", "mpcb200_destroy",
     "mpcb200_last_error", "mpcb200_upload_inputs", "mpcb200_solve_resident", "mpcb200_fetch_results",
     "mpcb200_device_controls", "mpcb200_ws_count", "mpcb200_ws_read", "mpcb200_ws_write", "mpcb200_run_phase",
-    "mpcb200_check_feasible", "mpcb200_time_phase", "mpcb200_set_timing", "mpcb200_set_stream", "mpcb200_set_option", "mpcb200_kernel_model", "mpcb200_solve_stream", "mpcb200_stats_get", "mpcb200_stats_reset", "mpcb200_export_controls", "mpcb200_flush_l2",
+    "mpcb200_check_feasible", "mpcb200_time_phase", "mpcb200_set_timing", "mpcb200_set_stream", "mpcb200_set_option", "mpcb200_kernel_model", "mpcb200_kernel_problem", "mpcb200_solve_stream", "mpcb200_stats_get", "mpcb200_stats_reset", "mpcb200_export_controls", "mpcb200_flush_l2",
     "mpcb200_resample", "mpcb200_get_horizon", "mpcb200_costmap_obstacles", "mpcb200_step_batch_costmap", "mpcb200_costmap_last_ms",
     "mpcb200_create_multi", "mpcb200_step_batch_multi", "mpcb200_multi_device_controls", "mpcb200_multi_fetch_controls", "mpcb200_multi_handle",
     "mpcb200_destroy_multi", "mpcb200_multi_last_error",
@@ -265,6 +266,7 @@ def load_library(path=None):
     lib.mpcb200_set_stream.argtypes = [vp, vp]
     lib.mpcb200_set_option.argtypes = [vp, C.c_int, C.c_int]
     lib.mpcb200_kernel_model.argtypes = [vp]
+    lib.mpcb200_kernel_problem.argtypes = [vp]
     lib.mpcb200_stats_get.argtypes = [vp, C.POINTER(Stats)]
     lib.mpcb200_stats_reset.argtypes = [vp]
     if path == LIB_PATH:
@@ -491,6 +493,10 @@ class BatchSolver:
     def kernel_model(self):
         """Model key of the last solve launch: MODEL_GENERIC or MODEL_UNI_POINT (see OPT_FORCE_GENERIC_MODEL)."""
         return self.lib.mpcb200_kernel_model(self.h)
+
+    def kernel_problem(self):
+        """Problem key of the last solve launch: PROBLEM_GENERIC or PROBLEM_FIXED_DT_QF (see OPT_FORCE_GENERIC_MODEL)."""
+        return self.lib.mpcb200_kernel_problem(self.h)
 
     def set_timing(self, phase_mask):
         """Phases bracketed by CUDA events inside a solve (bit p = phase p); default KKT only, 0x1f = all."""

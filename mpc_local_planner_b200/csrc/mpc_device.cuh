@@ -489,7 +489,7 @@ __device__ __forceinline__ int dev_eval(const Cfg& c, const WsLayout& L, double*
     {
         for (int w = 1; w < nw; ++w) evalacc_merge(a, sh.eacc[w]);
         int fin = 0;
-        sh.mu = eval_finish(c, L, W, a, true, &fin, budget_expired(sh.deadline));
+        sh.mu = eval_finish<MODEL>(c, L, W, a, true, &fin, budget_expired(sh.deadline));
         sh.fin = fin;
     }
     __syncthreads();
@@ -537,7 +537,7 @@ __device__ __forceinline__ void dev_linesearch(const Cfg& c, const WsLayout& L, 
     // histogram of the blocking step ratios (+ row count) -> threshold bin of the clipped rows -> primal step length
     for (int j = tid; j <= CLIP_BINS; j += nt) sh.hist[j] = 0;
     __syncthreads();
-    for (int k = tid; k < N; k += nt) ls_stage_steps(c, L, W, W, uprev_dt, k, a, sh.hist);
+    for (int k = tid; k < N; k += nt) ls_stage_steps<MODEL>(c, L, W, W, uprev_dt, k, a, sh.hist);
     __syncthreads();
     const int jt = clip_threshold_bin(sh.hist, sh.hist[CLIP_BINS]);  // same value in every thread
     for (int k = tid; k < N; k += nt) a.a_p = fmin(a.a_p, ls_stage_ap(L, W, k, jt));
@@ -600,10 +600,10 @@ __device__ __forceinline__ void dev_linesearch(const Cfg& c, const WsLayout& L, 
         for (int k = tid; k < N; k += nt) ls_stage_midpoint_fix(c, L, W, k);   // reads the old heading of stage k+1
     __syncthreads();
     const double a_dual = sh.a_dual;
-    for (int k = tid; k < N; k += nt) ls_stage_update(c, L, W, W, uprev_dt, k, alpha, a_dual);
+    for (int k = tid; k < N; k += nt) ls_stage_update<MODEL>(c, L, W, W, uprev_dt, k, alpha, a_dual);
     if (tid == 0)
     {
-        if (c.variable_dt) ASC(MPCB200_SC_DT) = ASC(MPCB200_SC_DT) + alpha * ASC(MPCB200_SC_DDT);
+        if (ModelTraits<MODEL>::variable_dt(c)) ASC(MPCB200_SC_DT) = ASC(MPCB200_SC_DT) + alpha * ASC(MPCB200_SC_DDT);
         ASC(MPCB200_SC_ALPHA) = alpha;
         ASC(MPCB200_SC_RHO) = rho;
         ASC(MPCB200_SC_ITER) = ASC(MPCB200_SC_ITER) + 1.0;

@@ -111,33 +111,62 @@ HD NOINL inline LinTerms lin_row_terms(double g, double s, double lam, double gm
     t.c0t = c0 * gdt; t.rst = rs * gdt; t.lamt = lam * gdt; t.sgtt = sig * gdt * gdt;
     return t;
 }
-template <int I>
+// the same row with dt fixed: the terms that do not involve gdt, each formed as in lin_row_terms
+struct LinTermsFixed { double r, rs, c0g, rsg, lamg, sgg, sgc; };
+HD NOINL inline LinTermsFixed lin_row_terms_fixed(double g, double s, double lam, double gmine, double gcross)
+{
+    LinTermsFixed t;
+    const double rs = 1.0 / s;
+    const double r = g + s, sig = lam * rs, c0 = sig * r;
+    t.r = r; t.rs = rs;
+    t.c0g = c0 * gmine; t.rsg = rs * gmine; t.lamg = lam * gmine;
+    t.sgg = sig * gmine * gmine; t.sgc = sig * gmine * gcross;
+    return t;
+}
+// DT = false: dt is fixed (gdt is not read); the dt terms are zero and are not accumulated
+template <int I, bool DT>
 HD inline void lin_row_accum(double g, double s, double lam, double gmine, double gdt, bool own, double gcross, double* H, double* g0,
                              double* g1, double* GL, double* hb, double* Cc, EvalAcc& acc, RowProd& rp)
 {
-    const LinTerms t = lin_row_terms(g, s, lam, gmine, gdt, gcross);
-    g0[3 + I] += t.c0g; g1[3 + I] += t.rsg; GL[3 + I] += t.lamg;
-    H[hidx(3 + I, 3 + I)] += t.sgg;
-    hb[3 + I] += t.sgt;
-    if (own)
+    if (DT)
     {
-        Cc[I] += t.sgc;
-        row_stats(acc, rp, t.r, s, lam);
-        acc.gt0 += t.c0t; acc.gt1 += t.rst; acc.gldt += t.lamt; acc.htt += t.sgtt;
+        const LinTerms t = lin_row_terms(g, s, lam, gmine, gdt, gcross);
+        g0[3 + I] += t.c0g; g1[3 + I] += t.rsg; GL[3 + I] += t.lamg;
+        H[hidx(3 + I, 3 + I)] += t.sgg;
+        hb[3 + I] += t.sgt;
+        if (own)
+        {
+            Cc[I] += t.sgc;
+            row_stats(acc, rp, t.r, s, lam);
+            acc.gt0 += t.c0t; acc.gt1 += t.rst; acc.gldt += t.lamt; acc.htt += t.sgtt;
+        }
+    }
+    else
+    {
+        const LinTermsFixed t = lin_row_terms_fixed(g, s, lam, gmine, gcross);
+        g0[3 + I] += t.c0g; g1[3 + I] += t.rsg; GL[3 + I] += t.lamg;
+        H[hidx(3 + I, 3 + I)] += t.sgg;
+        if (own)
+        {
+            Cc[I] += t.sgc;
+            row_stats(acc, rp, t.r, s, lam);
+        }
     }
 }
 
 // all linear rows that touch control component I of stage k <= N-2: bounds (slots 2I, 2I+1), own rate rows
 // (slots 4+2I, 5+2I) and the rate rows of stage k+1 (gather: their derivative wrt u_k)
-template <int I>
+template <int I, int MODEL>
 HD inline void lin_rows_component(const Cfg& c, const WsLayout& L, const double* W, double uprev_dt, int k, double dt, double u_i, double* H,
                                   double* g0, double* g1, double* GL, double* hb, double* Cc, EvalAcc& acc, RowProd& rp)
 {
+    using T_ = ModelTraits<MODEL>;
+    constexpr bool DT = T_::DT_TERMS;
     const int N = L.N;
     // control bounds
-    if (c.u_lb[I] > -MPCB200_INF) lin_row_accum<I>(c.u_lb[I] - u_i, AS(2 * I, k), ALAM(2 * I, k), -1.0, 0.0, true, 0.0, H, g0, g1, GL, hb, Cc, acc, rp);
-    if (c.u_ub[I] < MPCB200_INF) lin_row_accum<I>(u_i - c.u_ub[I], AS(2 * I + 1, k), ALAM(2 * I + 1, k), 1.0, 0.0, true, 0.0, H, g0, g1, GL, hb, Cc, acc, rp);
-    const bool has_lb = c.du_lb[I] > -MPCB200_INF, has_ub = c.du_ub[I] < MPCB200_INF;
+    if (T_::row_finite(c, 2 * I)) lin_row_accum<I, DT>(c.u_lb[I] - u_i, AS(2 * I, k), ALAM(2 * I, k), -1.0, 0.0, true, 0.0, H, g0, g1, GL, hb, Cc, acc, rp);
+    if (T_::row_finite(c, 2 * I + 1)) lin_row_accum<I, DT>(u_i - c.u_ub[I], AS(2 * I + 1, k), ALAM(2 * I + 1, k), 1.0, 0.0, true, 0.0, H, g0, g1, GL, hb, Cc, acc, rp);
+    const bool has_lb = T_::row_finite(c, 4 + 2 * I), has_ub = T_::row_finite(c, 5 + 2 * I);
     if (!has_lb && !has_ub) return;
     // own rate rows: Delta = u_k - u_{k-1}; k = 0 uses (u_prev, dt_prev) and is absent when dt_prev == 0
     if (!(k == 0 && uprev_dt == 0.0))
@@ -146,18 +175,18 @@ HD inline void lin_rows_component(const Cfg& c, const WsLayout& L, const double*
         const double T = (k >= 1) ? dt : uprev_dt;
         const double delta = u_i - um;
         const double cross = (k >= 1) ? 1.0 : 0.0;             // d/du_{k-1} exists only for k >= 1
-        const double dtf = (k >= 1 && c.variable_dt) ? 1.0 : 0.0;
-        if (has_lb) lin_row_accum<I>(-(delta - c.du_lb[I] * T), AS(4 + 2 * I, k), ALAM(4 + 2 * I, k), -1.0, dtf * c.du_lb[I], true, cross * 1.0, H, g0, g1, GL, hb, Cc, acc, rp);
-        if (has_ub) lin_row_accum<I>(delta - c.du_ub[I] * T, AS(5 + 2 * I, k), ALAM(5 + 2 * I, k), 1.0, -dtf * c.du_ub[I], true, cross * -1.0, H, g0, g1, GL, hb, Cc, acc, rp);
+        const double dtf = (k >= 1 && T_::variable_dt(c)) ? 1.0 : 0.0;
+        if (has_lb) lin_row_accum<I, DT>(-(delta - c.du_lb[I] * T), AS(4 + 2 * I, k), ALAM(4 + 2 * I, k), -1.0, dtf * c.du_lb[I], true, cross * 1.0, H, g0, g1, GL, hb, Cc, acc, rp);
+        if (has_ub) lin_row_accum<I, DT>(delta - c.du_ub[I] * T, AS(5 + 2 * I, k), ALAM(5 + 2 * I, k), 1.0, -dtf * c.du_ub[I], true, cross * -1.0, H, g0, g1, GL, hb, Cc, acc, rp);
     }
     // rate rows of stage k+1: Delta' = u_{k+1} - u_k (u_{N-1} := u_ref = 0); derivative wrt u_k is -sgn
     {
         const int kk = k + 1;
         const double un = (kk <= N - 2) ? AU(I, kk) : 0.0;
         const double delta = un - u_i;
-        const double dtf = c.variable_dt ? 1.0 : 0.0;
-        if (has_lb) lin_row_accum<I>(-(delta - c.du_lb[I] * dt), AS(4 + 2 * I, kk), ALAM(4 + 2 * I, kk), 1.0, dtf * c.du_lb[I], false, 0.0, H, g0, g1, GL, hb, Cc, acc, rp);
-        if (has_ub) lin_row_accum<I>(delta - c.du_ub[I] * dt, AS(5 + 2 * I, kk), ALAM(5 + 2 * I, kk), -1.0, -dtf * c.du_ub[I], false, 0.0, H, g0, g1, GL, hb, Cc, acc, rp);
+        const double dtf = T_::variable_dt(c) ? 1.0 : 0.0;
+        if (has_lb) lin_row_accum<I, DT>(-(delta - c.du_lb[I] * dt), AS(4 + 2 * I, kk), ALAM(4 + 2 * I, kk), 1.0, dtf * c.du_lb[I], false, 0.0, H, g0, g1, GL, hb, Cc, acc, rp);
+        if (has_ub) lin_row_accum<I, DT>(delta - c.du_ub[I] * dt, AS(5 + 2 * I, kk), ALAM(5 + 2 * I, kk), -1.0, -dtf * c.du_ub[I], false, 0.0, H, g0, g1, GL, hb, Cc, acc, rp);
     }
 }
 
@@ -168,8 +197,10 @@ HD inline void lin_rows_component(const Cfg& c, const WsLayout& L, const double*
 template <bool LINES = true, int MODEL = MODEL_GENERIC>
 HD inline void eval_stage(const Cfg& c, const WsLayout& L, double* W, double* G, double uprev_dt, int k, EvalAcc& acc)
 {
+    using T_ = ModelTraits<MODEL>;
     const int N = L.N, K = L.K;
     const double dt = ASC(MPCB200_SC_DT);
+    const bool vdt = T_::variable_dt(c);
     double H[15], g0[5], g1[5], GL[5], a3[3], Bm[6], e[3], Cc[2], hb[5], dvec[3];
 #pragma unroll
     for (int i = 0; i < 15; ++i) H[i] = 0.0;
@@ -227,11 +258,11 @@ HD inline void eval_stage(const Cfg& c, const WsLayout& L, double* W, double* G,
             }
         }
         // quadratic running cost (k = 0 state term is a constant: its gradient is never used since x_0 is fixed)
-        if (has_quadratic(c))
+        if (T_::quadratic(c))
         {
             // integral form: dt * (w_k l_x(x_k) + l_u(u_k)), w_k the state weight of the integration rule (left sum or
             // trapezoid, integral_state_weight); then the dt-gradient is w_k l_x + l_u and the w-dt cross Hessian its gradient
-            const bool integ = c.quadratic_integral_form != 0;
+            const bool integ = T_::integral(c);
             const double fx = integ ? integral_state_weight(c, N, k) : 1.0;
             const double wx = integ ? dt * fx : 1.0, wu = integ ? dt : 1.0;
             const double d[3] = {x[0] - xf[0], x[1] - xf[1], normalize_theta(x[2] - xf[2])};
@@ -248,7 +279,7 @@ HD inline void eval_stage(const Cfg& c, const WsLayout& L, double* W, double* G,
                     if (j >= i) H[hidx(i, j)] += wx * (c.Q[i * 3 + j] + c.Q[j * 3 + i]);
                 }
                 g0[i] += wx * gi; GL[i] += wx * gi;
-                if (integ && c.variable_dt) hb[i] += fx * gi;
+                if (integ && vdt) hb[i] += fx * gi;
             }
 #pragma unroll
             for (int i = 0; i < 2; ++i)
@@ -262,10 +293,10 @@ HD inline void eval_stage(const Cfg& c, const WsLayout& L, double* W, double* G,
                     if (j >= i) H[hidx(3 + i, 3 + j)] += wu * (c.R[i * 2 + j] + c.R[j * 2 + i]);
                 }
                 g0[3 + i] += wu * gi; GL[3 + i] += wu * gi;
-                if (integ && c.variable_dt) hb[3 + i] += gi;
+                if (integ && vdt) hb[3 + i] += gi;
             }
             acc.obj += wx * ox + wu * ou;
-            if (integ && c.variable_dt) { acc.gt0 += fx * ox + ou; acc.gldt += fx * ox + ou; }
+            if (integ && vdt) { acc.gt0 += fx * ox + ou; acc.gldt += fx * ox + ou; }
         }
         // Lagrangian terms of nu_k^T e_k
         const double fx_nu = nu[0] * J[0] + nu[1] * J[3] + nu[2] * J[6];
@@ -275,19 +306,19 @@ HD inline void eval_stage(const Cfg& c, const WsLayout& L, double* W, double* G,
         GL[0] += nu[0]; GL[1] += nu[1];
         GL[3] += dt * fu_nu0; GL[4] += dt * fu_nu1;
         H[hidx(3, 3)] += dt * Hc[3]; H[hidx(3, 4)] += dt * Hc[4]; H[hidx(4, 4)] += dt * Hc[5];
-        if (c.variable_dt) { hb[3] += fu_nu0; hb[4] += fu_nu1; }
+        if (vdt) { hb[3] += fu_nu0; hb[4] += fu_nu1; }
         if (!mid)
         {
             GL[2] += nu[2] + dt * fx_nu;
             H[hidx(2, 2)] += dt * Hc[0]; H[hidx(2, 3)] += dt * Hc[1]; H[hidx(2, 4)] += dt * Hc[2];
-            if (c.variable_dt) hb[2] += fx_nu;
+            if (vdt) hb[2] += fx_nu;
         }
         else
         {
             // theta_k enters through the mean heading with weight 1/2
             GL[2] += nu[2] + 0.5 * dt * fx_nu;
             H[hidx(2, 2)] += 0.25 * dt * Hc[0]; H[hidx(2, 3)] += 0.5 * dt * Hc[1]; H[hidx(2, 4)] += 0.5 * dt * Hc[2];
-            if (c.variable_dt) hb[2] += 0.5 * fx_nu;
+            if (vdt) hb[2] += 0.5 * fx_nu;
             // Hessian block between theta_{k+1} and (theta_k, u_k): q = (dt/4 Hc_tt, dt/2 Hc_t0, dt/2 Hc_t1).  It is condensed
             // into this stage with the linearised heading row d(theta_{k+1}) = r' dw_k + e~_2 + d~_2 d(dt), r = (1, B~_20, B~_21):
             // H += q r' + r q', Newton gradient += q e~_2, dt border += q d~_2 (exact; DESIGN.md "midpoint differences")
@@ -299,12 +330,12 @@ HD inline void eval_stage(const Cfg& c, const WsLayout& L, double* W, double* G,
 #pragma unroll
                 for (int j = i; j < 3; ++j) H[hidx(2 + i, 2 + j)] += q[i] * r[j] + r[i] * q[j];
                 g0[2 + i] += q[i] * e[2];
-                if (c.variable_dt) hb[2 + i] += q[i] * dvec[2];
+                if (vdt) hb[2 + i] += q[i] * dvec[2];
             }
         }
         // linear rows touching u_k (own bounds, own rate rows, rate rows of stage k+1)
-        lin_rows_component<0>(c, L, W, uprev_dt, k, dt, u[0], H, g0, g1, GL, hb, Cc, acc, rp);
-        lin_rows_component<1>(c, L, W, uprev_dt, k, dt, u[1], H, g0, g1, GL, hb, Cc, acc, rp);
+        lin_rows_component<0, MODEL>(c, L, W, uprev_dt, k, dt, u[0], H, g0, g1, GL, hb, Cc, acc, rp);
+        lin_rows_component<1, MODEL>(c, L, W, uprev_dt, k, dt, u[1], H, g0, g1, GL, hb, Cc, acc, rp);
     }
     else
     {
@@ -329,7 +360,7 @@ HD inline void eval_stage(const Cfg& c, const WsLayout& L, double* W, double* G,
             }
             acc.obj += o;
         }
-        if (has_trapezoid(c))
+        if (T_::trapezoid(c))
         {
             // end term of the trapezoidal rule: dt/2 * l_x(x_{N-1})
             const double fx = integral_state_weight(c, N, k);
@@ -347,25 +378,25 @@ HD inline void eval_stage(const Cfg& c, const WsLayout& L, double* W, double* G,
                     if (j >= i) H[hidx(i, j)] += dt * fx * (c.Q[i * 3 + j] + c.Q[j * 3 + i]);
                 }
                 g0[i] += dt * fx * gi; GL[i] += dt * fx * gi;
-                if (c.variable_dt) hb[i] += fx * gi;
+                if (vdt) hb[i] += fx * gi;
             }
             acc.obj += dt * fx * ox;
-            if (c.variable_dt) { acc.gt0 += fx * ox; acc.gldt += fx * ox; }
+            if (vdt) { acc.gt0 += fx * ox; acc.gldt += fx * ox; }
         }
-        if (has_mintime(c)) { acc.gt0 += (double)(N - 1); acc.gldt += (double)(N - 1); acc.obj += (double)(N - 1) * dt; }
+        if (T_::mintime(c)) { acc.gt0 += (double)(N - 1); acc.gldt += (double)(N - 1); acc.obj += (double)(N - 1) * dt; }
         for (int sl = 0; sl < 8; ++sl)
         {
-            if (!lin_row_active(c, N, k, sl, uprev_dt)) continue;
+            if (!lin_row_active<MODEL>(c, N, k, sl, uprev_dt)) continue;
             const int i = (sl < 4) ? (sl >> 1) : ((sl - 4) >> 1);
             double gu, gum, gdt;
             const double um = (sl >= 4) ? AU(i, k - 1) : 0.0;
-            const double g = lin_row(c, N, k, sl, 0.0, um, dt, uprev_dt, gu, gum, gdt);
+            const double g = lin_row<MODEL>(c, N, k, sl, 0.0, um, dt, uprev_dt, gu, gum, gdt);
             const double s = AS(sl, k), lam = ALAM(sl, k);
             const double rs = 1.0 / s, r = g + s, sig = lam * rs, c0 = sig * r;
             row_stats(acc, rp, r, s, lam);
-            acc.gt0 += c0 * gdt; acc.gt1 += rs * gdt; acc.gldt += lam * gdt; acc.htt += sig * gdt * gdt;
+            if (T_::DT_TERMS) { acc.gt0 += c0 * gdt; acc.gt1 += rs * gdt; acc.gldt += lam * gdt; acc.htt += sig * gdt * gdt; }
         }
-        if (ball_active(c))
+        if (T_::ball(c))
         {
             // terminal ball on x_{N-1} (slot BALL_SLOT): a nonlinear state row, handled like an obstacle row
             double gr[3], hd[6];
@@ -394,7 +425,7 @@ HD inline void eval_stage(const Cfg& c, const WsLayout& L, double* W, double* G,
         const double fx_nu_p = nup[0] * Jp[0] + nup[1] * Jp[3] + nup[2] * Jp[6];
         GL[2] += 0.5 * dt * fx_nu_p;
         H[hidx(2, 2)] += 0.25 * dt * Hp[0];
-        if (c.variable_dt) hb[2] += 0.5 * fx_nu_p;
+        if (vdt) hb[2] += 0.5 * fx_nu_p;
     }
     // via-points attached to this stage
     if (has_viapoints(c) && k >= 1 && k <= N - 2)
@@ -432,7 +463,7 @@ HD inline void eval_stage(const Cfg& c, const WsLayout& L, double* W, double* G,
             const double rs = 1.0 / s, r = g + s, sig = lam * rs, c0 = sig * r;
             row_stats(acc, rp, r, s, lam);
             const double gr[3] = {-gd[0], -gd[1], -gd[2]};
-            if (LINES && c.variable_dt && obstacle_is_dynamic(c, op))
+            if (LINES && vdt && obstacle_is_dynamic(c, op))
             {
                 // g = G(p - o - k dt v, theta): dg/ddt = -k grad_p g . v, d2g/dpose ddt = -k H_g v, d2g/ddt2 = k^2 v'H_g v  (H_g = -hd)
                 const double kk = (double)k, vx = op[5], vy = op[6];
@@ -483,13 +514,14 @@ HD inline void eval_stage(const Cfg& c, const WsLayout& L, double* W, double* G,
 // Returns the barrier parameter to finalise the gradients with; *finished is set when the instance terminates.
 // expired: the time budget of the solve (max_cpu_time) has run out.  It is tested after the iteration cap, so an instance stopped
 // here at iteration j holds exactly what a solve with max_iter = j leaves; only the status differs.
+template <int MODEL = MODEL_GENERIC>
 HD inline double eval_finish(const Cfg& c, const WsLayout& L, double* W, const EvalAcc& a, bool write, int* finished, bool expired = false)
 {
     double mu = ASC(MPCB200_SC_MU);
     const double tol = c.tol, mu_min = tol / 10.0;
     const int m_eq = (int)a.m_eq, m_in = (int)a.m_ineq;
     double dual_inf = a.dual_inf;
-    if (c.variable_dt) dual_inf = fmax(dual_inf, fabs(a.gldt));
+    if (ModelTraits<MODEL>::variable_dt(c)) dual_inf = fmax(dual_inf, fabs(a.gldt));
     const double e0 = scaled_error(dual_inf, a.prim_inf, a.sl_max, a.sl_min, a.sum_nu, a.sum_lam, m_eq, m_in, 0.0);
     double emu = scaled_error(dual_inf, a.prim_inf, a.sl_max, a.sl_min, a.sum_nu, a.sum_lam, m_eq, m_in, mu);
     const int iter = (int)ASC(MPCB200_SC_ITER);
@@ -552,9 +584,12 @@ HD inline void lsacc_init(LsAcc& a) { a.a_p = 1.0; a.a_d = 1.0; a.dphi_bar = a.c
 #define PART_BASE 1
 #define PART_OBST 2
 #define PART_ALL 3
+template <int MODEL = MODEL_GENERIC>
 HD inline void ls_stage_steps(const Cfg& c, const WsLayout& L, double* W, double* G, double uprev_dt, int k, LsAcc& acc, int* hist, int part = PART_ALL)
 {
+    using T_ = ModelTraits<MODEL>;
     const int N = L.N, K = L.K;
+    const bool vdt = T_::variable_dt(c);
     const double dt = ASC(MPCB200_SC_DT), mu = ASC(MPCB200_SC_MU), ddt = ASC(MPCB200_SC_DDT);
     const double delta = ASC(MPCB200_SC_DELTA);
     const double tau = (1.0 - mu > TAU_MIN) ? 1.0 - mu : TAU_MIN;
@@ -568,7 +603,7 @@ HD inline void ls_stage_steps(const Cfg& c, const WsLayout& L, double* W, double
     for (int sl = (part & PART_BASE) ? 0 : 8; sl < ((part & PART_OBST) ? 8 + K : 8); ++sl)
     {
         double g, gdz;
-        if (sl == BALL_SLOT && k == N - 1 && ball_active(c))
+        if (sl == BALL_SLOT && k == N - 1 && T_::ball(c))
         {
             double gr[3];
             g = ball_row(c, x, xf, gr, nullptr);
@@ -576,12 +611,12 @@ HD inline void ls_stage_steps(const Cfg& c, const WsLayout& L, double* W, double
         }
         else if (sl < 8)
         {
-            if (!lin_row_active(c, N, k, sl, uprev_dt)) { ADS(sl, k) = 0.0; GR0(sl, k) = 0.0; continue; }
+            if (!lin_row_active<MODEL>(c, N, k, sl, uprev_dt)) { ADS(sl, k) = 0.0; GR0(sl, k) = 0.0; continue; }
             const int i = (sl < 4) ? (sl >> 1) : ((sl - 4) >> 1);
             const double uk = (k <= N - 2) ? AU(i, k) : 0.0;
             const double um = (sl >= 4) ? ((k >= 1) ? AU(i, k - 1) : AIN(IN_UPREV + i)) : 0.0;
             double gu, gum, gdt;
-            g = lin_row(c, N, k, sl, uk, um, dt, uprev_dt, gu, gum, gdt);
+            g = lin_row<MODEL>(c, N, k, sl, uk, um, dt, uprev_dt, gu, gum, gdt);
             gdz = gu * du[i] + gdt * ddt;
             if (gum != 0.0) gdz += gum * ASTEP(3 + i, k - 1);
         }
@@ -593,7 +628,7 @@ HD inline void ls_stage_steps(const Cfg& c, const WsLayout& L, double* W, double
             g = GOG(4 * j + 0, k);
             gdz = GOG(4 * j + 1, k) * dx[0] + GOG(4 * j + 2, k) * dx[1] + GOG(4 * j + 3, k) * dx[2];
             const double* op = W + L.oOBST + oi * MPCB200_OBST_STRIDE;
-            if (c.variable_dt && obstacle_is_dynamic(c, op)) gdz += -(double)k * (GOG(4 * j + 1, k) * op[5] + GOG(4 * j + 2, k) * op[6]) * ddt;
+            if (vdt && obstacle_is_dynamic(c, op)) gdz += -(double)k * (GOG(4 * j + 1, k) * op[5] + GOG(4 * j + 2, k) * op[6]) * ddt;
         }
         const double s = AS(sl, k), lam = ALAM(sl, k);
         const double rs = 1.0 / s;
@@ -616,11 +651,11 @@ HD inline void ls_stage_steps(const Cfg& c, const WsLayout& L, double* W, double
     double dJ = 0.0;
     if (k <= N - 2)
     {
-        if (has_quadratic(c))
+        if (T_::quadratic(c))
         {
             const double d[3] = {x[0] - xf[0], x[1] - xf[1], normalize_theta(x[2] - xf[2])};
             const double u[2] = {AU(0, k), AU(1, k)};
-            const bool integ = c.quadratic_integral_form != 0;
+            const bool integ = T_::integral(c);
             const double fx = integ ? integral_state_weight(c, N, k) : 1.0;
             const double wx = integ ? ASC(MPCB200_SC_DT) * fx : 1.0, wu = integ ? ASC(MPCB200_SC_DT) : 1.0;
             double dlx = 0.0, dlu = 0.0, lx = 0.0, lu = 0.0;
@@ -628,26 +663,26 @@ HD inline void ls_stage_steps(const Cfg& c, const WsLayout& L, double* W, double
                 for (int j = 0; j < 3; ++j) { dlx += (c.Q[i * 3 + j] + c.Q[j * 3 + i]) * d[j] * dx[i]; lx += d[i] * c.Q[i * 3 + j] * d[j]; }
             for (int i = 0; i < 2; ++i)
                 for (int j = 0; j < 2; ++j) { dlu += (c.R[i * 2 + j] + c.R[j * 2 + i]) * u[j] * du[i]; lu += u[i] * c.R[i * 2 + j] * u[j]; }
-            dJ += wx * dlx + wu * dlu + ((integ && c.variable_dt) ? (fx * lx + lu) * ddt : 0.0);
+            dJ += wx * dlx + wu * dlu + ((integ && vdt) ? (fx * lx + lu) * ddt : 0.0);
         }
     }
     else
     {
-        if (has_mintime(c)) dJ += (double)(N - 1) * ddt;
+        if (T_::mintime(c)) dJ += (double)(N - 1) * ddt;
         if (has_terminal_cost(c))
         {
             const double d[3] = {x[0] - xf[0], x[1] - xf[1], normalize_theta(x[2] - xf[2])};
             for (int i = 0; i < 3; ++i)
                 for (int j = 0; j < 3; ++j) dJ += (c.Qf[i * 3 + j] + c.Qf[j * 3 + i]) * d[j] * dx[i];
         }
-        if (has_trapezoid(c))
+        if (T_::trapezoid(c))
         {
             const double fx = integral_state_weight(c, N, k);
             const double d[3] = {x[0] - xf[0], x[1] - xf[1], normalize_theta(x[2] - xf[2])};
             double dlx = 0.0, lx = 0.0;
             for (int i = 0; i < 3; ++i)
                 for (int j = 0; j < 3; ++j) { dlx += (c.Q[i * 3 + j] + c.Q[j * 3 + i]) * d[j] * dx[i]; lx += d[i] * c.Q[i * 3 + j] * d[j]; }
-            dJ += ASC(MPCB200_SC_DT) * fx * dlx + (c.variable_dt ? fx * lx * ddt : 0.0);
+            dJ += ASC(MPCB200_SC_DT) * fx * dlx + (vdt ? fx * lx * ddt : 0.0);
         }
     }
     if (has_viapoints(c) && k >= 1 && k <= N - 2)
@@ -680,11 +715,11 @@ HD inline void ls_stage_steps(const Cfg& c, const WsLayout& L, double* W, double
             }
         if (k >= 1 && k <= N - 2)
             for (int i = 0; i < 2; ++i) cv += 2.0 * ASTEP(3 + i, k - 1) * AKKT(MPCB200_K_C + i, k) * du[i];
-        if (c.variable_dt)  // border (the terminal record carries one only with the trapezoidal rule)
+        if (vdt)  // border (the terminal record carries one only with the trapezoidal rule)
 #pragma unroll
             for (int i = 0; i < 5; ++i)
                 if (i < nv) cv += 2.0 * ddt * AKKT(MPCB200_K_HB + i, k) * st[i];
-        if (c.variable_dt && k == N - 1) cv += ddt * ddt * (ASC(MPCB200_SC_HTT) + delta);
+        if (vdt && k == N - 1) cv += ddt * ddt * (ASC(MPCB200_SC_HTT) + delta);
         acc.curv += cv;
     }
 }
@@ -710,14 +745,16 @@ HD inline double ls_stage_ap(const WsLayout& L, const double* W, int k, int jt, 
 
 // objective contribution of stage k at (x, u, dt): quadratic running cost (k <= N-2; dt-weighted in integral form), terminal
 // cost and minimum-time term (k = N-1), via-points attached to the stage.  u is read for k <= N-2 only.
+template <int MODEL = MODEL_GENERIC>
 HD NOINL inline double stage_objective(const Cfg& c, const WsLayout& L, const double* W, int k, const double* x, const double* u, double dtt)
 {
+    using T_ = ModelTraits<MODEL>;
     const int N = L.N;
     const double xf[3] = {AIN(IN_XF), AIN(IN_XF + 1), AIN(IN_XF + 2)};
     double obj = 0.0;
     if (k <= N - 2)
     {
-        if (has_quadratic(c))
+        if (T_::quadratic(c))
         {
             const double d[3] = {x[0] - xf[0], x[1] - xf[1], normalize_theta(x[2] - xf[2])};
             double ox = 0.0, ou = 0.0;
@@ -729,13 +766,13 @@ HD NOINL inline double stage_objective(const Cfg& c, const WsLayout& L, const do
             for (int i = 0; i < 2; ++i)
 #pragma unroll
                 for (int j = 0; j < 2; ++j) ou += u[i] * c.R[i * 2 + j] * u[j];
-            const bool integ = c.quadratic_integral_form != 0;
+            const bool integ = T_::integral(c);
             obj += (integ ? dtt * integral_state_weight(c, N, k) : 1.0) * ox + (integ ? dtt : 1.0) * ou;
         }
     }
     else
     {
-        if (has_trapezoid(c))
+        if (T_::trapezoid(c))
         {
             const double d[3] = {x[0] - xf[0], x[1] - xf[1], normalize_theta(x[2] - xf[2])};
             double ox = 0.0;
@@ -745,7 +782,7 @@ HD NOINL inline double stage_objective(const Cfg& c, const WsLayout& L, const do
                 for (int j = 0; j < 3; ++j) ox += d[i] * c.Q[i * 3 + j] * d[j];
             obj += dtt * integral_state_weight(c, N, k) * ox;
         }
-        if (has_mintime(c)) obj += (double)(N - 1) * dtt;
+        if (T_::mintime(c)) obj += (double)(N - 1) * dtt;
         if (has_terminal_cost(c))
         {
             const double d[3] = {x[0] - xf[0], x[1] - xf[1], normalize_theta(x[2] - xf[2])};
@@ -778,8 +815,9 @@ struct TrialAcc { double obj, inf1, blog; };
 template <bool LINES = true, int MODEL = MODEL_GENERIC>
 HD inline void ls_stage_trial(const Cfg& c, const WsLayout& L, const double* W, const double* G, double uprev_dt, int k, double alpha, TrialAcc& acc, int part = PART_ALL)
 {
+    using T_ = ModelTraits<MODEL>;
     const int N = L.N, K = L.K;
-    const double dtt = ASC(MPCB200_SC_DT) + (c.variable_dt ? alpha * ASC(MPCB200_SC_DDT) : 0.0);
+    const double dtt = ASC(MPCB200_SC_DT) + (T_::variable_dt(c) ? alpha * ASC(MPCB200_SC_DDT) : 0.0);
     const double x[3] = {AX(0, k) + alpha * ASTEP(0, k), AX(1, k) + alpha * ASTEP(1, k), AX(2, k) + alpha * ASTEP(2, k)};
     const double xf[3] = {AIN(IN_XF), AIN(IN_XF + 1), AIN(IN_XF + 2)};
     double sc[2];
@@ -803,14 +841,14 @@ HD inline void ls_stage_trial(const Cfg& c, const WsLayout& L, const double* W, 
                               AX(2, k + 1) + alpha * ASTEP(2, k + 1)};
         acc.inf1 += fabs(x[0] + dtt * f[0] - xn[0]) + fabs(x[1] + dtt * f[1] - xn[1]) +
                     fabs(dtt * f[2] - normalize_theta(xn[2] - x[2]));
-        acc.obj += stage_objective(c, L, W, k, x, u, dtt);
+        acc.obj += stage_objective<MODEL>(c, L, W, k, x, u, dtt);
     }
-    else acc.obj += stage_objective(c, L, W, k, x, nullptr, dtt);
+    else acc.obj += stage_objective<MODEL>(c, L, W, k, x, nullptr, dtt);
     RowProd rp; rp.p = 1.0; rp.n = 0;
     const double oma = 1.0 - alpha;
     for (int sl = (part & PART_BASE) ? 0 : 8; sl < 8; ++sl)
     {
-        if (!lin_row_active(c, N, k, sl, uprev_dt)) continue;
+        if (!lin_row_active<MODEL>(c, N, k, sl, uprev_dt)) continue;
         const double s0 = AS(sl, k), ds = ADS(sl, k);
         double sn = s0 + alpha * ds;
         double res = oma * GR0(sl, k);           // g(alpha) + s + alpha ds, exact for linear rows
@@ -832,7 +870,7 @@ HD inline void ls_stage_trial(const Cfg& c, const WsLayout& L, const double* W, 
             acc.inf1 += fabs(c.min_obstacle_dist - dist + sn);
             rowprod_add(rp, sn, acc.blog);
         }
-    if ((part & PART_BASE) && k == N - 1 && ball_active(c))
+    if ((part & PART_BASE) && k == N - 1 && T_::ball(c))
     {
         double sn = AS(BALL_SLOT, k) + alpha * ADS(BALL_SLOT, k);
         if (sn < CLIP_FLOOR * AS(BALL_SLOT, k)) sn = CLIP_FLOOR * AS(BALL_SLOT, k);
@@ -859,6 +897,7 @@ HD inline void ls_stage_midpoint_fix(const Cfg& c, const WsLayout& L, double* W,
 }
 
 // accept the step: z, s, lambda, nu of stage k (reads and writes stage k only: safe to run lane-parallel in place)
+template <int MODEL = MODEL_GENERIC>
 HD inline void ls_stage_update(const Cfg& c, const WsLayout& L, const double* W, double* G, double uprev_dt, int k, double alpha, double a_dual, int part = PART_ALL)
 {
     const int N = L.N, K = L.K;
@@ -876,7 +915,7 @@ HD inline void ls_stage_update(const Cfg& c, const WsLayout& L, const double* W,
     for (int sl = (part & PART_BASE) ? 0 : 8; sl < ((part & PART_OBST) ? 8 + K : 8); ++sl)
     {
         bool act;
-        if (sl < 8) act = lin_row_active(c, N, k, sl, uprev_dt) || (sl == BALL_SLOT && k == N - 1 && ball_active(c));
+        if (sl < 8) act = lin_row_active<MODEL>(c, N, k, sl, uprev_dt) || (sl == BALL_SLOT && k == N - 1 && ModelTraits<MODEL>::ball(c));
         else act = (k >= 1 && k <= N - 2) && AOBS(sl - 8, k) >= 0;
         if (!act) continue;
         const double s0 = AS(sl, k), ds = ADS(sl, k), lam0 = ALAM(sl, k);

@@ -515,7 +515,7 @@ struct mpcb200_handle
     unsigned long long* d_smsync = nullptr;
     int max_ctas_per_sm = 0;         // MPCB200_OPT_CTAS_PER_SM: cap on the resident CTAs per SM of the solve kernel (0 = what fits)
     int force_generic_model = 0;     // MPCB200_OPT_FORCE_GENERIC_MODEL: never launch the variants compiled for one robot / footprint model
-    int last_model = MODEL_GENERIC;  // model key of the last solve launch (mpcb200_kernel_model)
+    int last_model = MODEL_GENERIC;  // kernel key of the last solve launch (mpcb200_kernel_model / mpcb200_kernel_problem)
     mpcb200_stats stats{};
     std::vector<cudaEvent_t> ev;     // pool of event pairs
     std::vector<int> ev_phase;
@@ -602,12 +602,14 @@ template <class K>
 static cudaError_t allow_smem(K kernel) { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_IMG_SMEM); }
 
 // ---- the kernel variants: one table per kernel.  The variants compiled for one robot / footprint model (MODEL_UNI_POINT) exist
-//      without the line-obstacle paths only (LINES = false); a request for one with them gets the generic variant. ----
+//      without the line-obstacle paths only (LINES = false); a request for one with them gets the generic variant.  The fixed-dt
+//      quadratic-form key (MODEL_UNI_POINT_QF) exists for the unbordered KKT only (EXT = false). ----
 using FusedKernel = decltype(&solve_fused_kernel<false, false, SMALL_GROUP_WARPS, MODEL_GENERIC>);
 template <int WARPS>
 static FusedKernel fused_shape_variant(bool lines, bool ext, int model)
 {
     if (lines) return ext ? solve_fused_kernel<true, true, WARPS, MODEL_GENERIC> : solve_fused_kernel<true, false, WARPS, MODEL_GENERIC>;
+    if (model == MODEL_UNI_POINT_QF && !ext) return solve_fused_kernel<false, false, WARPS, MODEL_UNI_POINT_QF>;
     if (model == MODEL_UNI_POINT) return ext ? solve_fused_kernel<false, true, WARPS, MODEL_UNI_POINT> : solve_fused_kernel<false, false, WARPS, MODEL_UNI_POINT>;
     return ext ? solve_fused_kernel<false, true, WARPS, MODEL_GENERIC> : solve_fused_kernel<false, false, WARPS, MODEL_GENERIC>;
 }
@@ -619,6 +621,7 @@ using PhaseKernel = decltype(&phase_kernel<false, MODEL_GENERIC>);
 static PhaseKernel phase_variant(bool lines, int model)
 {
     if (lines) return phase_kernel<true, MODEL_GENERIC>;
+    if (model == MODEL_UNI_POINT_QF) return phase_kernel<false, MODEL_UNI_POINT_QF>;
     return model == MODEL_UNI_POINT ? phase_kernel<false, MODEL_UNI_POINT> : phase_kernel<false, MODEL_GENERIC>;
 }
 
@@ -703,7 +706,7 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
     CKC(cudaMalloc(&h->d_counters, CNT_WORDS * 8)); CKC(cudaMemsetAsync(h->d_counters, 0, CNT_WORDS * 8, h->stream));
     CKC(allow_smem(kkt_warp_kernel<false>)); CKC(allow_smem(kkt_warp_kernel<true>));
     for (const bool lines : {false, true})
-        for (const int model : {MODEL_GENERIC, MODEL_UNI_POINT})
+        for (const int model : {MODEL_GENERIC, MODEL_UNI_POINT, MODEL_UNI_POINT_QF})
         {
             CKC(allow_smem(phase_variant(lines, model)));
             for (const bool ext : {false, true})
@@ -786,12 +789,14 @@ static int group_threads(const mpcb200_handle* h)
     const int gw = (h->cfg.n + 31) / 32;
     return 32 * (gw < MAX_GROUP_WARPS ? gw : MAX_GROUP_WARPS);   // a lane per stage
 }
-// robot model / footprint key of the evaluation and line-search code a launch runs (ModelTraits).  The specialised variants exist for
-// the kernels without the rarely used obstacle paths only (LINES = false).
+// robot model / footprint / problem key of the evaluation and line-search code a launch runs (ModelTraits).  The specialised variants
+// exist for the kernels without the rarely used obstacle paths only (LINES = false).
 static int kernel_model(const mpcb200_handle* h, const IoBuffers& io)
 {
+    if (io.has_lines || h->force_generic_model) return MODEL_GENERIC;
+    if (qf_key_matches(h->cfg)) return MODEL_UNI_POINT_QF;
     const bool uni_point = h->cfg.robot_type == MPCB200_ROBOT_UNICYCLE && h->cfg.footprint_type == MPCB200_FOOTPRINT_POINT;
-    return (uni_point && !io.has_lines && !h->force_generic_model) ? MODEL_UNI_POINT : MODEL_GENERIC;
+    return uni_point ? MODEL_UNI_POINT : MODEL_GENERIC;
 }
 static int image_words(const mpcb200_handle* h, const InputPtrs& in)
 {
@@ -1271,7 +1276,8 @@ extern "C" int mpcb200_set_option(mpcb200_handle* h, int option, int value)
     return set_err(h, MPCB200_E_INVALID, "unknown option or value");
 }
 
-extern "C" int mpcb200_kernel_model(const mpcb200_handle* h) { return h ? h->last_model : MPCB200_E_INVALID; }
+extern "C" int mpcb200_kernel_model(const mpcb200_handle* h) { return h ? model_key_of(h->last_model) : MPCB200_E_INVALID; }
+extern "C" int mpcb200_kernel_problem(const mpcb200_handle* h) { return h ? problem_key_of(h->last_model) : MPCB200_E_INVALID; }
 
 extern "C" int mpcb200_set_timing(mpcb200_handle* h, unsigned phase_mask)
 {
