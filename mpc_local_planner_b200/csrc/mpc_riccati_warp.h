@@ -323,8 +323,8 @@ HD inline double rw_colprod(const double* cur, const RwColProg& cp, const RwColC
 {
     return (rw_at(cur, cp.m[0]) * co.f[0] + rw_at(cur, cp.m[1]) * co.f[1]) + (rw_at(cur, cp.m[2]) * co.f[2] + rw_at(cur, cp.mo));
 }
-// phase B: one entry from the table.  la, lb, ld = MM'_vv (read in phase A, while `cur` still holds MM'); the reciprocal of
-// its determinant is formed here, beside the table loads.  *ok: inertia of the pivot (the same in every lane).
+// phase B: one entry from the table.  la, lb, ld = MM'_vv and idet = 1 / det(MM'_vv) (formed in phase A, while `cur` still
+// holds MM').
 template <bool EXT>
 HD inline double rw_entry(const double* tt, const RwEntProg& en, const RwEntCoef& co, double la, double lb, double ld, double idet)
 {
@@ -519,6 +519,8 @@ struct RwLane
     RwEntProg en[RW<EXT>::EPL];
     RwEntCoef ec[RW<EXT>::EPL];
     double la, lb, ld;         // pivot block of the stage matrix in `cur`
+    double idet;               // ... the reciprocal of its determinant
+    bool pok;                  // ... and its inertia test
     RwMap out, in;             // scan operands
     double y[5];
 };
@@ -567,8 +569,12 @@ HD inline int kkt_warp_attempt(Exec& ex, const Cfg& c, int N, double* recs, doub
     bool ok = true;
     for (int k = N - 2; k >= 0; --k)
     {
-        // ---- phase A: column products of MM_{k+1}; the pivot block is read while `cur` still holds MM_{k+1} ----
+        // ---- phase A: column products of MM_{k+1}; the pivot block is read while `cur` still holds MM_{k+1}, and the
+        //      reciprocal of its determinant is formed here: its latency overlaps the column products and the barrier
+        //      instead of delaying the last operation of every entry in phase B ----
         ex.each([&](int lane, RwLane<EXT>& ls) {
+            ls.la = cur[T::oVV]; ls.lb = cur[T::oVV + 1]; ls.ld = cur[T::oVV + 2];
+            ls.pok = rw_pivot(ls.la, ls.lb, ls.ld, &ls.idet);
 #pragma unroll
             for (int s = 0; s < T2::SLA; ++s)
             {
@@ -577,22 +583,19 @@ HD inline int kkt_warp_attempt(Exec& ex, const Cfg& c, int N, double* recs, doub
                 const double v = rw_colprod(cur, ls.cp[s], co);
                 if (ls.cp[s].active) tt[ls.cp[s].out] = v;
             }
-            ls.la = cur[T::oVV]; ls.lb = cur[T::oVV + 1]; ls.ld = cur[T::oVV + 2];
         });
         ex.sync();
         // ---- phase B: entries of MM_k; raw coefficients of the next stage ----
         double* mk = mms + (size_t)k * T::MSTR;
         const double* rnext = recs + (size_t)(k > 0 ? k - 1 : 0) * RSTR;
         ex.each([&](int lane, RwLane<EXT>& ls) {
-            double idet;
-            const bool okk = rw_pivot(ls.la, ls.lb, ls.ld, &idet);
-            ok = ok && okk;
+            ok = ok && ls.pok;
 #pragma unroll
             for (int s = 0; s < T::EPL; ++s)
             {
                 RwEntCoef co;
                 rw_coef_ent(ls.en[s], ls.ec[s], delta, co);
-                const double v = rw_entry<EXT>(tt, ls.en[s], co, ls.la, ls.lb, ls.ld, idet);
+                const double v = rw_entry<EXT>(tt, ls.en[s], co, ls.la, ls.lb, ls.ld, ls.idet);
                 if (ls.en[s].active) { cur[ls.en[s].e] = v; mk[ls.en[s].e] = v; }
             }
 #pragma unroll
