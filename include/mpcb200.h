@@ -299,6 +299,50 @@ int mpcb200_check_feasible(mpcb200_handle* h, int B, const mpcb200_costmaps* map
 /* device time (ms, CUDA events around the three kernels) of the last mpcb200_costmap_obstacles call */
 double mpcb200_costmap_last_ms(const mpcb200_handle* h);
 
+/* ---- device arrays in and out, stream-ordered: for callers whose data already lives on the GPU --------------------------------
+ * mpcb200_step_batch_async, mpcb200_step_batch_costmap_async and mpcb200_check_feasible_async take the arguments of
+ * mpcb200_step_batch, mpcb200_step_batch_costmap and mpcb200_check_feasible (without solve_time_s) and compute the same results,
+ * instance by instance and bit for bit.  The differences:
+ *   - Device memory.  Every array argument, including the arrays inside mpcb200_obstacles, mpcb200_viapoints and
+ *     mpcb200_costmaps, is device memory of the handle's device (checked with cudaPointerGetAttributes: anything else is
+ *     E_INVALID and nothing is enqueued).  The structs themselves and their scalar fields (max_per_instance, size_x, size_y,
+ *     resolution) stay on the host.  Maps, footprints and trajectories are read in place; the other inputs are copied device to
+ *     device into the handle's staging arrays, and the results are copied out of them.
+ *   - No host access and no waiting.  The call reads no array content on the host; it enqueues its work on the handle's stream
+ *     (mpcb200_set_stream) and returns.  The results are valid in stream order, and the caller keeps the arrays alive until then.
+ *   - The return code reports argument and launch errors only; the per-instance outcomes are in `status`, on the device.
+ *   - No events and no solve_time_s: bracket the work with events of your own.  The solve kernel's cycle counters stay on the
+ *     device and are folded into mpcb200_stats by the next call that synchronises the stream (mpcb200_stats_get included).
+ *     h2d_bytes and d2h_bytes count host copies only, so these calls leave them unchanged; launches_total counts enqueued launches
+ *     (a CUDA graph replay enqueues none).
+ *   - Shared state.  The blocking and the _async calls share the batch state of the handle (warm start, the order by the previous
+ *     solve's iteration counts, mpcb200_reset): mixed in stream order they give the results of the all-blocking sequence.
+ *   - Line obstacles.  The host does not scan the obstacle types, so the caller declares them: flags & MPCB200_ASYNC_LINE_OBSTACLES
+ *     when the lists may hold MPCB200_OBST_LINE (the kernels with the line paths also serve midpoint differences and dynamic
+ *     obstacles, chosen from the configuration as in mpcb200_step_batch).  An undeclared line obstacle makes its instance
+ *     MPCB200_STATUS_INVALID_INPUT; the other instances are unaffected.
+ *   - MPCB200_OPT_SOLVE_MODE 1 queues the iterations by polling from the host: the two solves return E_UNSUPPORTED in that mode.
+ *   - CUDA graphs.  The calls are capturable: set the stream once outside the capture (mpcb200_set_stream drains it), make one
+ *     call with the same shapes outside the capture (the staging arrays and the costmap scratch grow there, and CUDA loads the
+ *     kernels), then capture.  A call that would have to grow a buffer during a capture returns E_INVALID and leaves the capture
+ *     intact.  Decisions the host takes at enqueue time are frozen in the graph: the kernel variant, the CTA count and whether
+ *     the queue is ordered by the previous solve (which needs the same B as the previous batch solve and B > the SM count).
+ */
+#define MPCB200_ASYNC_LINE_OBSTACLES 1u   /* the obstacle lists may hold MPCB200_OBST_LINE */
+int mpcb200_step_batch_async(mpcb200_handle* h, int B, const double* x0, const double* xf, const double* u_prev, double u_prev_dt,
+                             const mpcb200_obstacles* obst, const mpcb200_viapoints* vp, const double* x_init,
+                             const unsigned char* reinit, unsigned flags,
+                             double* u_seq, double* x_seq, double* dt_out, int* status, double* kkt_err, int* iters);
+int mpcb200_step_batch_costmap_async(mpcb200_handle* h, int B, const double* x0, const double* xf, const double* u_prev,
+                                     double u_prev_dt, const mpcb200_costmaps* maps, double behind_robot_dist, int max_per_instance,
+                                     const mpcb200_viapoints* vp, const double* x_init, const unsigned char* reinit,
+                                     double* u_seq, double* x_seq, double* dt_out, int* status, double* kkt_err, int* iters,
+                                     int* obst_found);
+/* x_seq = NULL: the trajectories of the last solve of the handle, in stream order (also after an _async solve) */
+int mpcb200_check_feasible_async(mpcb200_handle* h, int B, const mpcb200_costmaps* maps, const double* x_seq, int n_poses,
+                                 const double* footprint_xy, int n_footprint, double inscribed_radius, double circumscribed_radius,
+                                 double min_resolution_angular, int look_ahead_idx, unsigned char* feasible);
+
 void mpcb200_destroy(mpcb200_handle* h);
 
 /* Last error message of this handle (or of create() when h == NULL). Never NULL. */

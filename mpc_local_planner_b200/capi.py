@@ -36,6 +36,7 @@ OPT_ORDER_BY_HISTORY = 6
 OPT_FORCE_GENERIC_MODEL = 7
 MODEL_GENERIC, MODEL_UNI_POINT = 0, 1
 PROBLEM_GENERIC, PROBLEM_FIXED_DT_QF = 0, 1
+ASYNC_LINE_OBSTACLES = 1
 SOLVE_FUSED, SOLVE_PHASED = 0, 1
 NUM_PHASES = 5
 K_H, K_G, K_A, K_B, K_E, K_C, K_HB, K_D = 0, 15, 20, 23, 29, 32, 34, 39
@@ -204,6 +205,7 @@ EXPORTS = [
     "mpcb200_resample", "mpcb200_get_horizon", "mpcb200_costmap_obstacles", "mpcb200_step_batch_costmap", "mpcb200_costmap_last_ms",
     "mpcb200_create_multi", "mpcb200_step_batch_multi", "mpcb200_multi_device_controls", "mpcb200_multi_fetch_controls", "mpcb200_multi_handle",
     "mpcb200_destroy_multi", "mpcb200_multi_last_error",
+    "mpcb200_step_batch_async", "mpcb200_step_batch_costmap_async", "mpcb200_check_feasible_async",
 ]
 
 
@@ -269,6 +271,13 @@ def load_library(path=None):
     lib.mpcb200_kernel_problem.argtypes = [vp]
     lib.mpcb200_stats_get.argtypes = [vp, C.POINTER(Stats)]
     lib.mpcb200_stats_reset.argtypes = [vp]
+    # device-memory entry points: every array is a device pointer
+    lib.mpcb200_step_batch_async.argtypes = [vp, C.c_int, vp, vp, vp, C.c_double, C.POINTER(Obstacles), C.POINTER(ViaPoints), vp, vp, C.c_uint,
+                                             vp, vp, vp, vp, vp, vp]
+    lib.mpcb200_step_batch_costmap_async.argtypes = [vp, C.c_int, vp, vp, vp, C.c_double, C.POINTER(Costmaps), C.c_double, C.c_int,
+                                                     C.POINTER(ViaPoints), vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.mpcb200_check_feasible_async.argtypes = [vp, C.c_int, C.POINTER(Costmaps), vp, C.c_int, vp, C.c_int, C.c_double, C.c_double,
+                                                 C.c_double, C.c_int, vp]
     if path == LIB_PATH:
         _LIB = lib
     return lib
@@ -276,6 +285,31 @@ def load_library(path=None):
 
 class SolverError(RuntimeError):
     pass
+
+
+def _tensor_ptr(t, name, dtype, device, shape, optional=False):
+    """Device pointer of a torch CUDA tensor for the _async entry points (None for an absent optional array).  Raises ValueError
+    unless the tensor is contiguous, of `dtype` and on `device`; `shape`: the expected shape, None for a free dimension."""
+    import torch
+    if t is None:
+        if optional:
+            return None
+        raise ValueError(f"{name} is required")
+    if not isinstance(t, torch.Tensor):
+        raise ValueError(f"{name} must be a torch CUDA tensor, got {type(t).__name__}")
+    if not t.is_cuda or t.device.index != device:
+        raise ValueError(f"{name} must be on cuda:{device}, got {t.device}")
+    if t.dtype != dtype:
+        raise ValueError(f"{name} must be {dtype}, got {t.dtype}")
+    if not t.is_contiguous():
+        raise ValueError(f"{name} must be contiguous")
+    if len(shape) != t.dim() or any(s is not None and s != d for s, d in zip(shape, t.shape)):
+        raise ValueError(f"{name} has shape {tuple(t.shape)}, expected {tuple('*' if s is None else s for s in shape)}")
+    return t.data_ptr()
+
+
+def _as_ptr(addr, ctype):
+    return C.cast(C.c_void_p(addr), C.POINTER(ctype)) if addr else None
 
 
 class BatchSolver:
@@ -294,6 +328,8 @@ class BatchSolver:
             raise SolverError(f"mpcb200_create failed ({rc}): {msg}")
         self.h = h
         self.B = 0
+        self.device = int(device)
+        self.stream = 0   # cudaStream_t the handle runs on (0: its own stream), see set_stream
 
     def close(self):
         if getattr(self, "h", None):
@@ -484,8 +520,119 @@ class BatchSolver:
         self._check(self.lib.mpcb200_run_phase(self.h, phase, B or self.B), "mpcb200_run_phase")
 
     def set_stream(self, cuda_stream):
-        """Run on the caller's CUDA stream (an integer cudaStream_t, e.g. torch.cuda.Stream().cuda_stream); 0 restores."""
+        """Run on the caller's CUDA stream (an integer cudaStream_t, e.g. torch.cuda.Stream().cuda_stream); 0 restores.  Drains
+        the previous stream: call it outside a CUDA graph capture."""
         self._check(self.lib.mpcb200_set_stream(self.h, C.c_void_p(int(cuda_stream) if cuda_stream else None)), "mpcb200_set_stream")
+        self.stream = int(cuda_stream) if cuda_stream else 0
+
+    # device arrays in and out (mpcb200_*_async) -----------------------------------------------------------------------------
+    def _async_prologue(self):
+        """The _async calls enqueue on the handle's stream, which must be torch's current stream (set_stream(
+        torch.cuda.current_stream().cuda_stream) once, outside any capture): torch's work and the solve are then ordered."""
+        import torch
+        cur = torch.cuda.current_stream(self.device).cuda_stream
+        if self.stream == 0 or int(cur) != self.stream:
+            raise SolverError("the handle's stream is not torch.cuda.current_stream(): call set_stream(torch.cuda.current_stream()"
+                              ".cuda_stream) outside any graph capture first")
+        return torch
+
+    def _async_outputs(self, torch, B, out, keys):
+        """result tensors: out[key] where given (checked), else new tensors (from the graph's pool during a capture)"""
+        N, dev = self.N, f"cuda:{self.device}"
+        spec = dict(u_seq=((B, N, 2), torch.float64), x_seq=((B, N, 3), torch.float64), dt=((B,), torch.float64),
+                    status=((B,), torch.int32), kkt_err=((B,), torch.float64), iters=((B,), torch.int32),
+                    obst_found=((B,), torch.int32), feasible=((B,), torch.uint8))
+        res = {}
+        for k in keys:
+            shape, dtype = spec[k]
+            t = out.get(k) if out is not None else None
+            if t is None:
+                t = torch.empty(shape, dtype=dtype, device=dev)
+            _tensor_ptr(t, f"out[{k!r}]", dtype, self.device, shape)
+            res[k] = t
+        return res
+
+    def _async_common(self, torch, x0, xf, u_prev, viapoints, x_init, reinit):
+        B = x0.shape[0] if hasattr(x0, "shape") and len(x0.shape) == 2 else None
+        f64, dev = torch.float64, self.device
+        p = dict(x0=_tensor_ptr(x0, "x0", f64, dev, (B, 3)), xf=_tensor_ptr(xf, "xf", f64, dev, (B, 3)),
+                 u_prev=_tensor_ptr(u_prev, "u_prev", f64, dev, (B, 2), optional=True),
+                 x_init=_tensor_ptr(x_init, "x_init", f64, dev, (B, self.N, 3), optional=True),
+                 reinit=_tensor_ptr(reinit, "reinit", torch.uint8, dev, (B,), optional=True))
+        v = None
+        if viapoints is not None:
+            vc, vpz = viapoints
+            _tensor_ptr(vc, "viapoints count", torch.int32, dev, (B,))
+            _tensor_ptr(vpz, "viapoints poses", f64, dev, (B, None, 3))
+            v = ViaPoints(int(vpz.shape[1]), _as_ptr(vc.data_ptr(), C.c_int), _as_ptr(vpz.data_ptr(), C.c_double))
+        return B, p, v
+
+    def _maps(self, torch, cost, origin, resolution):
+        _tensor_ptr(cost, "cost", torch.uint8, self.device, (None, None, None))
+        B = cost.shape[0]
+        _tensor_ptr(origin, "origin", torch.float64, self.device, (B, 2))
+        return B, Costmaps(cost.shape[2], cost.shape[1], float(resolution), _as_ptr(origin.data_ptr(), C.c_double),
+                           _as_ptr(cost.data_ptr(), C.c_ubyte))
+
+    def step_async(self, x0, xf, u_prev=None, u_prev_dt=0.0, obstacles=None, viapoints=None, x_init=None, reinit=None,
+                   line_obstacles=False, out=None):
+        """step() on torch CUDA tensors (mpcb200_step_batch_async): float64 states, int32 counts and types, uint8 reinit;
+        obstacles = (count [B], type [B, M], params [B, M, OBST_STRIDE]), viapoints = (count [B], poses [B, V, 3]).  Enqueued on
+        the handle's stream, which must be torch's current stream; returns without waiting.  line_obstacles: the lists may hold
+        OBST_LINE (undeclared, such an instance ends INVALID_INPUT).  Returns a dict of CUDA tensors: u_seq, x_seq, dt, status,
+        kkt_err, iters (written in stream order; `out`: tensors to write them into)."""
+        torch = self._async_prologue()
+        B, p, v = self._async_common(torch, x0, xf, u_prev, viapoints, x_init, reinit)
+        o = None
+        if obstacles is not None:
+            oc, ot, op = obstacles
+            _tensor_ptr(oc, "obstacle count", torch.int32, self.device, (B,))
+            _tensor_ptr(ot, "obstacle types", torch.int32, self.device, (B, None))
+            M = ot.shape[1]
+            _tensor_ptr(op, "obstacle params", torch.float64, self.device, (B, M, OBST_STRIDE))
+            o = Obstacles(int(M), _as_ptr(oc.data_ptr(), C.c_int), _as_ptr(ot.data_ptr(), C.c_int), _as_ptr(op.data_ptr(), C.c_double))
+        res = self._async_outputs(torch, B, out, ("u_seq", "x_seq", "dt", "status", "kkt_err", "iters"))
+        rc = self.lib.mpcb200_step_batch_async(
+            self.h, B, p["x0"], p["xf"], p["u_prev"], float(u_prev_dt), C.byref(o) if o else None, C.byref(v) if v else None,
+            p["x_init"], p["reinit"], ASYNC_LINE_OBSTACLES if line_obstacles else 0,
+            *(res[k].data_ptr() for k in ("u_seq", "x_seq", "dt", "status", "kkt_err", "iters")))
+        self._check(rc, "mpcb200_step_batch_async")
+        self.B = B
+        return res
+
+    def step_from_costmaps_async(self, x0, xf, cost, origin, resolution, behind_robot_dist, max_per_instance, u_prev=None, u_prev_dt=0.0,
+                                 viapoints=None, x_init=None, reinit=None, out=None):
+        """step_from_costmaps() on torch CUDA tensors (mpcb200_step_batch_costmap_async): cost [B, size_y, size_x] uint8 (read in
+        place, any alignment), origin [B, 2] float64, the rest as step_async.  Returns step_async's dict plus obst_found [B]."""
+        torch = self._async_prologue()
+        Bm, m = self._maps(torch, cost, origin, resolution)
+        B, p, v = self._async_common(torch, x0, xf, u_prev, viapoints, x_init, reinit)
+        if B != Bm:
+            raise ValueError(f"{Bm} maps for {B} robots")
+        keys = ("u_seq", "x_seq", "dt", "status", "kkt_err", "iters", "obst_found")
+        res = self._async_outputs(torch, B, out, keys)
+        rc = self.lib.mpcb200_step_batch_costmap_async(
+            self.h, B, p["x0"], p["xf"], p["u_prev"], float(u_prev_dt), C.byref(m), float(behind_robot_dist), int(max_per_instance),
+            C.byref(v) if v else None, p["x_init"], p["reinit"], *(res[k].data_ptr() for k in keys))
+        self._check(rc, "mpcb200_step_batch_costmap_async")
+        self.B = B
+        return res
+
+    def check_feasible_async(self, cost, origin, resolution, footprint, inscribed_radius, min_resolution_angular, look_ahead_idx=-1,
+                             x_seq=None, circumscribed_radius=0.0, out=None):
+        """check_feasible() on torch CUDA tensors (mpcb200_check_feasible_async): maps as step_from_costmaps_async, footprint
+        [n_fp, 2] float64, x_seq [B, n, 3] float64 or None (the trajectories of the last solve, in stream order).  Returns
+        {"feasible": uint8 [B]}."""
+        torch = self._async_prologue()
+        B, m = self._maps(torch, cost, origin, resolution)
+        fp = _tensor_ptr(footprint, "footprint", torch.float64, self.device, (None, 2))
+        xs = _tensor_ptr(x_seq, "x_seq", torch.float64, self.device, (B, None, 3), optional=True)
+        res = self._async_outputs(torch, B, out, ("feasible",))
+        rc = self.lib.mpcb200_check_feasible_async(
+            self.h, B, C.byref(m), xs, x_seq.shape[1] if x_seq is not None else 0, fp if footprint.shape[0] else None, footprint.shape[0],
+            float(inscribed_radius), float(circumscribed_radius), float(min_resolution_angular), int(look_ahead_idx), res["feasible"].data_ptr())
+        self._check(rc, "mpcb200_check_feasible_async")
+        return res
 
     def set_option(self, option, value):
         self._check(self.lib.mpcb200_set_option(self.h, option, value), "mpcb200_set_option")

@@ -103,7 +103,11 @@ struct InputPtrs
 struct OutputPtrs { double* u_seq; double* x_seq; double* dt; int* status; double* kkt; int* iters; double* u_packed; };
 
 // ---- scatter the compact input arrays into an instance block (inputs of instance `src`), one warp.  Returns false
-//      (warp-uniform) when an input that will be used is not finite: the instance is reported as INVALID_INPUT. ----
+//      (warp-uniform) when an input that will be used is not finite: the instance is reported as INVALID_INPUT.  Kernels
+//      compiled without the line-obstacle paths (LINES = false) also reject a line obstacle: they would take its distance as
+//      that of a point.  The blocking entry points never launch them on lines (they scan the types on the host); the
+//      device-memory entry points choose the variant from what the caller declares, so an undeclared line ends here. ----
+template <bool LINES>
 __device__ __forceinline__ bool scatter_one(const WsLayout& L, double* W, const InputPtrs& in, int64_t src, int lane, double* xinit_dst)
 {
     const int N = L.N;
@@ -132,11 +136,14 @@ __device__ __forceinline__ bool scatter_one(const WsLayout& L, double* W, const 
         if (!long_list) W[L.oOBST + i] = v;
         ok = ok && isfinite(v);
     }
+    // (unrolled as the compiler unrolls the check with line obstacles: the cheaper check without them was unrolled 16 times,
+    // which moved all code behind it in the instruction-fetch-bound solve kernels and cost 0.5 % of a cold solve)
+#pragma unroll 4
     for (int i = lane; i < nob; i += 32)
     {
         const int t = in.obst_type[src * in.obst_max + i];
         if (!long_list) W[L.oOTYPE + i] = (double)t;
-        ok = ok && t >= MPCB200_OBST_POINT && t <= MPCB200_OBST_LINE;
+        ok = ok && t >= MPCB200_OBST_POINT && t <= (LINES ? MPCB200_OBST_LINE : MPCB200_OBST_CIRCLE);
     }
     for (int i = lane; i < nvp * 3; i += 32) { const double v = in.vp_poses[src * in.vp_max * 3 + i]; W[L.oVP + i] = v; ok = ok && isfinite(v); }
     if (in.x_init && xinit_dst)

@@ -21,6 +21,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <initializer_list>
 #include <string>
 #include <vector>
 
@@ -39,6 +40,9 @@
 #define CNT_INST 8         // instances solved by the fused kernel
 #define CNT_GATE 9         // SM cycles CTAs waited at the phase gates (MPCB200_OPT_SM_PHASE_SYNC)
 #define CNT_WORDS 16
+// behind the CNT_WORDS counters: CNT_WORDS doubles, the counters of the device-memory solves already folded per launch
+// (fold_counters_kernel): cycle words as cycles per CTA of their own launch, the other words as counts
+#define CNT_BYTES (CNT_WORDS * 8 * 2)
 
 // ---- kernel: inputs of a batch into the instance blocks (phased path; the fused kernel scatters into shared memory itself) ----
 __global__ void scatter_inputs_kernel(WsLayout L, double* ws, int B, InputPtrs in)
@@ -46,7 +50,7 @@ __global__ void scatter_inputs_kernel(WsLayout L, double* ws, int B, InputPtrs i
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= B) return;
     double* W = ws + (int64_t)warp * L.stride;
-    const bool ok = scatter_one(L, W, in, warp, lane, W + L.oXINIT);
+    const bool ok = scatter_one<true>(L, W, in, warp, lane, W + L.oXINIT);   // (the phased mode serves the blocking calls only)
     if (lane == 0) ASC(MPCB200_SC_VALID) = ok ? 1.0 : 0.0;
 }
 
@@ -345,7 +349,7 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
         // ---- inputs ----
         if (wid == 0)
         {
-            const bool ok = scatter_one(L, W, a.in, inst, lane, nullptr);
+            const bool ok = scatter_one<LINES>(L, W, a.in, inst, lane, nullptr);
             if (lane == 0) { s_valid = ok; ASC(MPCB200_SC_VALID) = ok ? 1.0 : 0.0; if (!ok) mark_invalid(L, W); }
         }
         __syncthreads();
@@ -456,6 +460,18 @@ __global__ void resample_unpack_kernel(WsLayout L, double* ws, const double* rec
     ASC(MPCB200_SC_DT) = resample_serial(n_old, r + MPCB200_SCAL_WORDS, r + MPCB200_SCAL_WORDS + 3 * n_old, r[MPCB200_SC_DT], L.N, W + L.oX, W + L.oU);
 }
 
+
+// ---- the counters of a solve launch that no host synchronise follows: a mean per CTA needs the grid of its own launch, and
+//      launches of different grids may accumulate before the next synchronising call reads them ----
+__global__ void fold_counters_kernel(unsigned long long* raw, int grid)
+{
+    const int i = threadIdx.x;
+    if (i >= CNT_WORDS) return;
+    double* fold = reinterpret_cast<double*>(raw + CNT_WORDS);
+    const bool cycles = (i >= CNT_CYC && i < CNT_CYC + MPCB200_NUM_PHASES) || i == CNT_GATE;
+    fold[i] += cycles ? (double)raw[i] / (double)grid : (double)raw[i];
+    raw[i] = 0ull;
+}
 
 __global__ void flush_kernel(double* buf, size_t n)
 {
@@ -625,6 +641,43 @@ static PhaseKernel phase_variant(bool lines, int model)
     return model == MODEL_UNI_POINT ? phase_kernel<false, MODEL_UNI_POINT> : phase_kernel<false, MODEL_GENERIC>;
 }
 
+// Where the arrays of a call live.  Host: the blocking calls copy them in and out and synchronise the stream.  Device: the
+// _async calls copy device to device on the stream, read no array content on the host and do not wait.
+enum class Mem { Host, Device };
+
+// A buffer of the handle has to grow: allocating (and the synchronise before freeing) would end a CUDA graph capture on the
+// handle's stream, so a call that needs it during a capture fails instead and asks for a warm-up.
+static int check_growth_allowed(mpcb200_handle* h, const char* what)
+{
+    cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+    CK(cudaStreamIsCapturing(h->stream, &st));
+    if (st != cudaStreamCaptureStatusNone)
+        return set_err(h, MPCB200_E_INVALID, std::string(what) + " must grow while the stream is capturing a CUDA graph: make the same call "
+                                             "once with the same shapes before the capture (warm-up)");
+    return 0;
+}
+
+// The arrays a device-memory entry point takes must be device (or managed) memory of the handle's device: the kernels read the
+// maps, footprints and trajectories in place, where a host pointer would be a fault rather than an error.  Null entries are the
+// optional arrays the caller left out.
+static int check_device_arrays(mpcb200_handle* h, const char* what, std::initializer_list<const void*> arrays)
+{
+    for (const void* p : arrays)
+    {
+        if (!p) continue;
+        cudaPointerAttributes a{};
+        if (cudaPointerGetAttributes(&a, p) != cudaSuccess)
+        {
+            cudaGetLastError();   // (not sticky; cleared so that no later check reports it)
+            return set_err(h, MPCB200_E_INVALID, std::string(what) + ": an array pointer is not known to CUDA");
+        }
+        if ((a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != h->device)
+            return set_err(h, MPCB200_E_INVALID, std::string(what) + ": every array must be device memory of the handle's device (device " +
+                                                 std::to_string(h->device) + ")");
+    }
+    return 0;
+}
+
 // frees the arrays of `io` and empties it (nothing held)
 static void io_release(IoBuffers& io)
 {
@@ -641,6 +694,7 @@ static int io_reserve(mpcb200_handle* h, IoBuffers& io, size_t rows, int obst_pe
 {
     const int m = (obst_per_instance > MAX_OBST && obst_per_instance <= MAX_OBST_LIST) ? obst_per_instance : MAX_OBST;
     if (rows <= io.rows && m <= io.obst_m) return 0;
+    if (int rc = check_growth_allowed(h, "the staging arrays")) return rc;
     CK(cudaStreamSynchronize(h->stream));   // work queued on the stream may still read the arrays
     if (rows > io.rows)
     {
@@ -703,7 +757,7 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
     }
     CKC(cudaMalloc(&h->d_nactive, 8)); CKC(cudaMalloc(&h->d_queue, 4)); CKC(cudaMalloc(&h->d_smsync, 1024 * 8)); CKC(cudaMalloc(&h->d_prev_iters, B * 4)); CKC(cudaMalloc(&h->d_prev_status, B * 4)); CKC(cudaMalloc(&h->d_order, B * 4));
     CKC(cudaMalloc(&h->d_origin, 8));
-    CKC(cudaMalloc(&h->d_counters, CNT_WORDS * 8)); CKC(cudaMemsetAsync(h->d_counters, 0, CNT_WORDS * 8, h->stream));
+    CKC(cudaMalloc(&h->d_counters, CNT_BYTES)); CKC(cudaMemsetAsync(h->d_counters, 0, CNT_BYTES, h->stream));
     CKC(allow_smem(kkt_warp_kernel<false>)); CKC(allow_smem(kkt_warp_kernel<true>));
     for (const bool lines : {false, true})
         for (const int model : {MODEL_GENERIC, MODEL_UNI_POINT, MODEL_UNI_POINT_QF})
@@ -850,11 +904,16 @@ static bool has_line_obstacles(size_t B, const mpcb200_obstacles* obst)
     return false;
 }
 
-// host -> device copies of the inputs of `B` instances into `io`, and the description of what it now holds (io.in, io.uprev_dt,
-// io.has_lines).  The arguments are checked before anything is copied.
+// copies of the inputs of `B` instances into `io` (host -> device, or device -> device: `mem`), and the description of what it now
+// holds (io.in, io.uprev_dt, io.has_lines).  The arguments are checked before anything is copied.  The line-obstacle kernel
+// variant follows the configuration and the obstacle types: scanned on the host for host arrays, declared by the caller
+// (`flags & MPCB200_ASYNC_LINE_OBSTACLES`) for device arrays.  h2d_bytes counts the host copies only.
 static int load_inputs(mpcb200_handle* h, IoBuffers& io, int B, const double* x0, const double* xf, const double* u_prev, double u_prev_dt,
-                       const mpcb200_obstacles* obst, const mpcb200_viapoints* vp, const double* x_init, const unsigned char* reinit)
+                       const mpcb200_obstacles* obst, const mpcb200_viapoints* vp, const double* x_init, const unsigned char* reinit,
+                       Mem mem = Mem::Host, unsigned flags = 0u)
 {
+    const cudaMemcpyKind kind = mem == Mem::Host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
+    const long long counted = mem == Mem::Host ? 1 : 0;
     if (!x0 || !xf) return set_err(h, MPCB200_E_INVALID, "x0 and xf are required");
     const bool with_obst = obst && obst->count && obst->max_per_instance > 0, with_vp = vp && vp->count && vp->max_per_instance > 0;
     if (with_obst && obst->max_per_instance > MAX_OBST_LIST) return set_err(h, MPCB200_E_UNSUPPORTED, "more than 2048 obstacles per instance");
@@ -863,32 +922,33 @@ static int load_inputs(mpcb200_handle* h, IoBuffers& io, int B, const double* x0
     if (int rc = io_reserve(h, io, io.rows, with_obst ? obst->max_per_instance : 0)) return rc;
     const size_t n = (size_t)B, N = (size_t)h->cfg.n;
     InputPtrs in{io.x0, io.xf, io.uprev, nullptr, io.obst_type, io.obst, 0, nullptr, io.vp, 0, nullptr, nullptr};
-    if (u_prev) { CK(cudaMemcpyAsync(io.uprev, u_prev, n * 2 * 8, cudaMemcpyHostToDevice, h->stream)); h->stats.h2d_bytes += (long long)(n * 16); }
+    if (u_prev) { CK(cudaMemcpyAsync(io.uprev, u_prev, n * 2 * 8, kind, h->stream)); h->stats.h2d_bytes += counted * (long long)(n * 16); }
     else CK(cudaMemsetAsync(io.uprev, 0, n * 2 * 8, h->stream));
-    CK(cudaMemcpyAsync(io.x0, x0, n * 3 * 8, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(io.xf, xf, n * 3 * 8, cudaMemcpyHostToDevice, h->stream));
-    h->stats.h2d_bytes += (long long)(n * 6 * 8);
+    CK(cudaMemcpyAsync(io.x0, x0, n * 3 * 8, kind, h->stream));
+    CK(cudaMemcpyAsync(io.xf, xf, n * 3 * 8, kind, h->stream));
+    h->stats.h2d_bytes += counted * (long long)(n * 6 * 8);
     bool lines = is_midpoint(h->cfg);
     if (with_obst)
     {
         const size_t M = (size_t)obst->max_per_instance;
-        CK(cudaMemcpyAsync(io.obst_count, obst->count, n * 4, cudaMemcpyHostToDevice, h->stream));
-        CK(cudaMemcpyAsync(io.obst_type, obst->type, n * M * 4, cudaMemcpyHostToDevice, h->stream));
-        CK(cudaMemcpyAsync(io.obst, obst->params, n * M * MPCB200_OBST_STRIDE * 8, cudaMemcpyHostToDevice, h->stream));
-        h->stats.h2d_bytes += (long long)(n * 4 + n * M * 4 + n * M * MPCB200_OBST_STRIDE * 8);
+        CK(cudaMemcpyAsync(io.obst_count, obst->count, n * 4, kind, h->stream));
+        CK(cudaMemcpyAsync(io.obst_type, obst->type, n * M * 4, kind, h->stream));
+        CK(cudaMemcpyAsync(io.obst, obst->params, n * M * MPCB200_OBST_STRIDE * 8, kind, h->stream));
+        h->stats.h2d_bytes += counted * (long long)(n * 4 + n * M * 4 + n * M * MPCB200_OBST_STRIDE * 8);
         in.obst_count = io.obst_count; in.obst_max = (int)M;
-        lines = lines || h->cfg.enable_dynamic_obstacles || has_line_obstacles(n, obst);
+        const bool line_obstacles = mem == Mem::Host ? has_line_obstacles(n, obst) : (flags & MPCB200_ASYNC_LINE_OBSTACLES) != 0u;
+        lines = lines || h->cfg.enable_dynamic_obstacles || line_obstacles;
     }
     if (with_vp)
     {
         const size_t V = (size_t)vp->max_per_instance;
-        CK(cudaMemcpyAsync(io.vp_count, vp->count, n * 4, cudaMemcpyHostToDevice, h->stream));
-        CK(cudaMemcpyAsync(io.vp, vp->poses, n * V * 3 * 8, cudaMemcpyHostToDevice, h->stream));
-        h->stats.h2d_bytes += (long long)(n * 4 + n * V * 24);
+        CK(cudaMemcpyAsync(io.vp_count, vp->count, n * 4, kind, h->stream));
+        CK(cudaMemcpyAsync(io.vp, vp->poses, n * V * 3 * 8, kind, h->stream));
+        h->stats.h2d_bytes += counted * (long long)(n * 4 + n * V * 24);
         in.vp_count = io.vp_count; in.vp_max = (int)V;
     }
-    if (x_init && io.xinit) { CK(cudaMemcpyAsync(io.xinit, x_init, n * N * 3 * 8, cudaMemcpyHostToDevice, h->stream)); in.x_init = io.xinit; h->stats.h2d_bytes += (long long)(n * N * 24); }
-    if (reinit && io.reinit) { CK(cudaMemcpyAsync(io.reinit, reinit, n, cudaMemcpyHostToDevice, h->stream)); in.reinit = io.reinit; h->stats.h2d_bytes += (long long)n; }
+    if (x_init && io.xinit) { CK(cudaMemcpyAsync(io.xinit, x_init, n * N * 3 * 8, kind, h->stream)); in.x_init = io.xinit; h->stats.h2d_bytes += counted * (long long)(n * N * 24); }
+    if (reinit && io.reinit) { CK(cudaMemcpyAsync(io.reinit, reinit, n, kind, h->stream)); in.reinit = io.reinit; h->stats.h2d_bytes += counted * (long long)n; }
     io.in = in;
     io.uprev_dt = u_prev_dt;
     io.has_lines = lines;
@@ -992,17 +1052,23 @@ static int solve_phased(mpcb200_handle* h, int B, int force_cold)
     return 0;
 }
 
-// fold the cycle counters of the fused kernel into the per-phase statistics: average time a CTA spent in each phase
+// fold the cycle counters of the fused kernel into the per-phase statistics: average time a CTA spent in each phase.  The raw
+// counters hold the launches since the last fold, all of the grid h->fused_grid (a blocking solve folds its own launch); the
+// device-memory solves have folded theirs on the device already.
 static int collect_fused_counters(mpcb200_handle* h)
 {
-    unsigned long long cnt[CNT_WORDS];
+    unsigned long long cnt[2 * CNT_WORDS];
+    static_assert(sizeof(cnt) == CNT_BYTES, "raw counters + folded counters");
     CK(cudaMemcpy(cnt, h->d_counters, sizeof(cnt), cudaMemcpyDeviceToHost));
+    double fold[CNT_WORDS];
+    memcpy(fold, cnt + CNT_WORDS, sizeof(fold));
     const double per_cta = h->fused_grid > 0 ? 1.0 / ((double)h->fused_grid * (double)h->clock_khz) : 0.0;  // cycles -> ms per CTA
-    for (int p = 0; p < MPCB200_NUM_PHASES; ++p) h->stats.ms[p] += (double)cnt[CNT_CYC + p] * per_cta;
-    h->stats.gate_ms += (double)cnt[CNT_GATE] * per_cta;
-    h->stats.kkt_instances += (long long)cnt[CNT_KKT_INST];
-    h->stats.kkt_sweeps += (long long)cnt[CNT_KKT_SWEEPS];
-    h->stats.launches[MPCB200_PHASE_KKT] += (long long)cnt[CNT_KKT_INST];
+    const double to_ms = 1.0 / (double)h->clock_khz;
+    for (int p = 0; p < MPCB200_NUM_PHASES; ++p) h->stats.ms[p] += (double)cnt[CNT_CYC + p] * per_cta + fold[CNT_CYC + p] * to_ms;
+    h->stats.gate_ms += (double)cnt[CNT_GATE] * per_cta + fold[CNT_GATE] * to_ms;
+    h->stats.kkt_instances += (long long)cnt[CNT_KKT_INST] + (long long)fold[CNT_KKT_INST];
+    h->stats.kkt_sweeps += (long long)cnt[CNT_KKT_SWEEPS] + (long long)fold[CNT_KKT_SWEEPS];
+    h->stats.launches[MPCB200_PHASE_KKT] += (long long)cnt[CNT_KKT_INST] + (long long)fold[CNT_KKT_INST];
     CK(cudaMemsetAsync(h->d_counters, 0, sizeof(cnt), h->stream));
     return 0;
 }
@@ -1013,6 +1079,17 @@ static int check_budget_mode(mpcb200_handle* h)
     if (h->budget_ns && h->solve_mode == 1)
         return set_err(h, MPCB200_E_UNSUPPORTED, "max_cpu_time (a time budget) needs the fused solve kernel: MPCB200_OPT_SOLVE_MODE 1 "
                                                  "(one launch per phase) has no budget; set the option to 0 or max_cpu_time to -1");
+    return 0;
+}
+
+// The solve of a batch on the device arrays: one launch of the persistent kernel.  Without a host synchronise behind it (the
+// device-memory calls), its counters are folded on the device with the launch's own grid.
+static int launch_solve_async(mpcb200_handle* h, const IoBuffers& io, int total)
+{
+    if (int rc = launch_fused(h, io, total, 0, 0)) return rc;
+    fold_counters_kernel<<<1, CNT_WORDS, 0, h->stream>>>(h->d_counters, h->fused_grid);
+    h->stats.launches_total += 1;
+    CK(cudaGetLastError());
     return 0;
 }
 
@@ -1032,17 +1109,21 @@ static int timed_launch(mpcb200_handle* h, const IoBuffers& io, int total, int q
     return collect_fused_counters(h);
 }
 
-// results of `B` instances from `io` to the host (a null destination is skipped)
-static int fetch_outputs(mpcb200_handle* h, const IoBuffers& io, int B, double* u_seq, double* x_seq, double* dt_out, int* status, double* kkt_err, int* iters)
+// results of `B` instances from `io` to the host, then a synchronise (Mem::Host), or into device arrays in stream order
+// (Mem::Device; d2h_bytes counts the host copies only).  A null destination is skipped.
+static int fetch_outputs(mpcb200_handle* h, const IoBuffers& io, int B, double* u_seq, double* x_seq, double* dt_out, int* status, double* kkt_err, int* iters,
+                         Mem mem = Mem::Host)
 {
     const size_t n = (size_t)B, N = (size_t)h->cfg.n;
-    if (u_seq) { CK(cudaMemcpyAsync(u_seq, io.useq, n * N * 16, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(n * N * 16); }
-    if (x_seq) { CK(cudaMemcpyAsync(x_seq, io.xseq, n * N * 24, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(n * N * 24); }
-    if (dt_out) { CK(cudaMemcpyAsync(dt_out, io.dt, n * 8, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(n * 8); }
-    if (status) { CK(cudaMemcpyAsync(status, io.status, n * 4, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(n * 4); }
-    if (kkt_err) { CK(cudaMemcpyAsync(kkt_err, io.kkt, n * 8, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(n * 8); }
-    if (iters) { CK(cudaMemcpyAsync(iters, io.iters, n * 4, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)(n * 4); }
-    CK(cudaStreamSynchronize(h->stream));
+    const cudaMemcpyKind kind = mem == Mem::Host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
+    const long long counted = mem == Mem::Host ? 1 : 0;
+    if (u_seq) { CK(cudaMemcpyAsync(u_seq, io.useq, n * N * 16, kind, h->stream)); h->stats.d2h_bytes += counted * (long long)(n * N * 16); }
+    if (x_seq) { CK(cudaMemcpyAsync(x_seq, io.xseq, n * N * 24, kind, h->stream)); h->stats.d2h_bytes += counted * (long long)(n * N * 24); }
+    if (dt_out) { CK(cudaMemcpyAsync(dt_out, io.dt, n * 8, kind, h->stream)); h->stats.d2h_bytes += counted * (long long)(n * 8); }
+    if (status) { CK(cudaMemcpyAsync(status, io.status, n * 4, kind, h->stream)); h->stats.d2h_bytes += counted * (long long)(n * 4); }
+    if (kkt_err) { CK(cudaMemcpyAsync(kkt_err, io.kkt, n * 8, kind, h->stream)); h->stats.d2h_bytes += counted * (long long)(n * 8); }
+    if (iters) { CK(cudaMemcpyAsync(iters, io.iters, n * 4, kind, h->stream)); h->stats.d2h_bytes += counted * (long long)(n * 4); }
+    if (mem == Mem::Host) CK(cudaStreamSynchronize(h->stream));
     return 0;
 }
 
@@ -1325,7 +1406,7 @@ extern "C" int mpcb200_stats_reset(mpcb200_handle* h)
     if (!h) return MPCB200_E_INVALID;
     memset(&h->stats, 0, sizeof(h->stats));
     CK(cudaSetDevice(h->device));
-    CK(cudaMemsetAsync(h->d_counters, 0, CNT_WORDS * 8, h->stream));
+    CK(cudaMemsetAsync(h->d_counters, 0, CNT_BYTES, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return 0;
 }
@@ -1338,10 +1419,12 @@ extern "C" int mpcb200_export_controls(mpcb200_handle* h, void* dst_dev)
     return 0;
 }
 // costmap -> point obstacles on the device.  Poses come from the host (host_pose) or are already on the device (dev_pose: the x0 array
-// of a step); lists go to d_count / d_type / d_params ([B], [B][M], [B][M][7]; nullptr: scratch of this call).
+// of a step); lists go to d_count / d_type / d_params ([B], [B][M], [B][M][7]; nullptr: scratch of this call).  Host maps
+// (Mem::Host) are copied into the scratch and the kernels are bracketed by the events c0 / c1; device maps are read in place,
+// with no events.
 struct CostmapOut { int* count; int* found; int* type; double* params; };
 static int costmap_run(mpcb200_handle* h, int B, const mpcb200_costmaps* maps, const double* host_pose, const double* dev_pose, double behind_robot_dist,
-                       int max_per_instance, int* d_count, int* d_type, double* d_params, CostmapOut* out)
+                       int max_per_instance, int* d_count, int* d_type, double* d_params, CostmapOut* out, Mem mem = Mem::Host)
 {
     if (B < 1 || !maps || !maps->cost || !maps->origin || max_per_instance < 1)
         return set_err(h, MPCB200_E_INVALID, "costmap_obstacles: B >= 1, maps, poses and output arrays are required");
@@ -1351,10 +1434,12 @@ static int costmap_run(mpcb200_handle* h, int B, const mpcb200_costmaps* maps, c
     const int ncg = (int)((W + MARK_COLS - 1) / MARK_COLS); // 16-column groups per row
     const int Wp = ncg * MARK_COLS;                      // mask row pitch: sixteen columns per marking thread
     const size_t mask_words = (size_t)B * nrb * Wp;
-    const size_t need = (size_t)B * W * H + 16 + (size_t)B * 5 * 8 + 2 * (size_t)B * 4 + (size_t)B * M * (MPCB200_OBST_STRIDE * 8 + 4) +
+    const size_t map_bytes = mem == Mem::Host ? (size_t)B * W * H : 0;
+    const size_t need = map_bytes + 16 + (size_t)B * 5 * 8 + 2 * (size_t)B * 4 + (size_t)B * M * (MPCB200_OBST_STRIDE * 8 + 4) +
                         mask_words * 4 + 512;
     if (need > h->cm_cap)
     {
+        if (int rc = check_growth_allowed(h, "the costmap scratch")) return rc;
         CK(cudaStreamSynchronize(h->stream));
         if (h->d_cm) cudaFree(h->d_cm);
         h->d_cm = nullptr; h->cm_cap = 0;
@@ -1371,26 +1456,37 @@ static int costmap_run(mpcb200_handle* h, int B, const mpcb200_costmaps* maps, c
     int* d_found = (int*)p; p += (size_t)B * 4;
     int* s_type = (int*)p; p += (size_t)B * M * 4;
     p = (char*)(((uintptr_t)p + 15) & ~(uintptr_t)15);
-    unsigned char* d_cost = (unsigned char*)p;            // 16-byte aligned (16-byte loads when size_x % 16 == 0)
     if (!d_count) d_count = s_count;
     if (!d_type) d_type = s_type;
     if (!d_params) d_params = s_params;
-    CK(cudaMemcpyAsync(d_cost, maps->cost, (size_t)B * W * H, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(d_origin, maps->origin, (size_t)B * 16, cudaMemcpyHostToDevice, h->stream));
-    if (host_pose) CK(cudaMemcpyAsync(d_pose, host_pose, (size_t)B * 24, cudaMemcpyHostToDevice, h->stream));
-    h->stats.h2d_bytes += (long long)((size_t)B * W * H + (size_t)B * (host_pose ? 40 : 16));
-    CostmapArgs a{maps->size_x, maps->size_y, maps->resolution, behind_robot_dist, d_cost, d_origin, host_pose ? d_pose : dev_pose};
+    const unsigned char* cost = maps->cost;
+    const double* origin = maps->origin;
+    if (mem == Mem::Host)
+    {
+        unsigned char* d_cost = (unsigned char*)p;        // 16-byte aligned
+        CK(cudaMemcpyAsync(d_cost, maps->cost, (size_t)B * W * H, cudaMemcpyHostToDevice, h->stream));
+        CK(cudaMemcpyAsync(d_origin, maps->origin, (size_t)B * 16, cudaMemcpyHostToDevice, h->stream));
+        if (host_pose) CK(cudaMemcpyAsync(d_pose, host_pose, (size_t)B * 24, cudaMemcpyHostToDevice, h->stream));
+        h->stats.h2d_bytes += (long long)((size_t)B * W * H + (size_t)B * (host_pose ? 40 : 16));
+        cost = d_cost; origin = d_origin;
+    }
+    CostmapArgs a{maps->size_x, maps->size_y, maps->resolution, behind_robot_dist, cost, origin, host_pose ? d_pose : dev_pose};
     const dim3 grid_mark((unsigned)(((size_t)B * ncg * nrb + 255) / 256));
     // slots behind count[b] are padding: zeroed, so that what goes back to the caller (and on into step_batch) is defined
     CK(cudaMemsetAsync(d_type, 0, (size_t)B * M * 4, h->stream));
     CK(cudaMemsetAsync(d_params, 0, (size_t)B * M * MPCB200_OBST_STRIDE * 8, h->stream));
-    CK(cudaEventRecord(h->c0, h->stream));
-    if (W % 16 == 0) costmap_mark_kernel<16><<<grid_mark, 256, 0, h->stream>>>(a, B, nrb, ncg, Wp, d_mask);
-    else if (W % 4 == 0) costmap_mark_kernel<4><<<grid_mark, 256, 0, h->stream>>>(a, B, nrb, ncg, Wp, d_mask);
+    if (mem == Mem::Host) CK(cudaEventRecord(h->c0, h->stream));
+    // Load width: every row of every map must start VB-aligned, i.e. size_x and the base address are multiples of VB.  The
+    // scratch copy is 16-byte aligned; a caller's map may start anywhere.  No load reaches past the B size_y size_x bytes: tiles
+    // beyond the last map are not run (b < B), rows from size_y - 1 on are not loaded, and inside a row the 16-byte load covers
+    // columns c0..c0+15 < size_x (size_x % 16 == 0), the 4- and 1-byte loads test every word or byte against size_x.
+    const uintptr_t base = (uintptr_t)cost;
+    if (W % 16 == 0 && base % 16 == 0) costmap_mark_kernel<16><<<grid_mark, 256, 0, h->stream>>>(a, B, nrb, ncg, Wp, d_mask);
+    else if (W % 4 == 0 && base % 4 == 0) costmap_mark_kernel<4><<<grid_mark, 256, 0, h->stream>>>(a, B, nrb, ncg, Wp, d_mask);
     else costmap_mark_kernel<1><<<grid_mark, 256, 0, h->stream>>>(a, B, nrb, ncg, Wp, d_mask);
     costmap_emit_kernel<<<B, 256, 0, h->stream>>>(a, B, nrb, Wp, d_mask, max_per_instance, d_count, d_found, d_params, d_type);
     CK(cudaGetLastError());
-    CK(cudaEventRecord(h->c1, h->stream));
+    if (mem == Mem::Host) CK(cudaEventRecord(h->c1, h->stream));
     h->stats.launches_total += 2;
     out->count = d_count; out->found = d_found; out->type = d_type; out->params = d_params;
     return 0;
@@ -1448,19 +1544,28 @@ extern "C" int mpcb200_step_batch_costmap(mpcb200_handle* h, int B, const double
     return rc;
 }
 
-extern "C" int mpcb200_check_feasible(mpcb200_handle* h, int B, const mpcb200_costmaps* maps, const double* x_seq, int n_poses, const double* footprint_xy,
-                                      int n_footprint, double inscribed_radius, double circumscribed_radius, double min_resolution_angular,
-                                      int look_ahead_idx, unsigned char* feasible)
+// the arguments of a feasibility check; *n = poses per trajectory
+static int check_feasible_args(mpcb200_handle* h, int B, const mpcb200_costmaps* maps, const double* x_seq, int n_poses, const double* footprint_xy,
+                               int n_footprint, double inscribed_radius, double min_resolution_angular, const unsigned char* feasible, int* n)
 {
-    (void)circumscribed_radius;   // CostmapModel::footprintCost does not use it either
     if (!h) return MPCB200_E_INVALID;
     if (B < 1 || !maps || !maps->cost || !maps->origin || !feasible || n_footprint < 0 || (n_footprint > 0 && !footprint_xy))
         return set_err(h, MPCB200_E_INVALID, "check_feasible: B >= 1, maps, footprint and the output array are required");
     if (maps->size_x < 1 || maps->size_y < 1 || !(maps->resolution > 0)) return set_err(h, MPCB200_E_INVALID, "check_feasible: bad map geometry");
     if (!(inscribed_radius > 0) || !(min_resolution_angular > 0)) return set_err(h, MPCB200_E_INVALID, "check_feasible: inscribed_radius and min_resolution_angular must be > 0");
-    const int n = x_seq ? n_poses : h->cfg.n;
-    if (n < 1) return set_err(h, MPCB200_E_INVALID, "check_feasible: n_poses >= 1 required");
+    *n = x_seq ? n_poses : h->cfg.n;
+    if (*n < 1) return set_err(h, MPCB200_E_INVALID, "check_feasible: n_poses >= 1 required");
     if (!x_seq && (h->B < B)) return set_err(h, MPCB200_E_INVALID, "check_feasible: no solved batch of this size on the device (pass x_seq)");
+    return 0;
+}
+
+extern "C" int mpcb200_check_feasible(mpcb200_handle* h, int B, const mpcb200_costmaps* maps, const double* x_seq, int n_poses, const double* footprint_xy,
+                                      int n_footprint, double inscribed_radius, double circumscribed_radius, double min_resolution_angular,
+                                      int look_ahead_idx, unsigned char* feasible)
+{
+    (void)circumscribed_radius;   // CostmapModel::footprintCost does not use it either
+    int n = 0;
+    if (int rc = check_feasible_args(h, B, maps, x_seq, n_poses, footprint_xy, n_footprint, inscribed_radius, min_resolution_angular, feasible, &n)) return rc;
     CK(cudaSetDevice(h->device));
     const size_t W = (size_t)maps->size_x, H = (size_t)maps->size_y;
     const size_t need = (size_t)B * n * 24 + (size_t)B * 16 + (size_t)(n_footprint > 0 ? n_footprint : 1) * 16 + (size_t)B * W * H + (size_t)B + 256;
@@ -1494,6 +1599,82 @@ extern "C" int mpcb200_check_feasible(mpcb200_handle* h, int B, const mpcb200_co
 }
 
 extern "C" double mpcb200_costmap_last_ms(const mpcb200_handle* h) { return h ? h->costmap_ms : 0.0; }
+
+// ---- device-memory entry points: the paths above with device arrays, stream-ordered, no host synchronise ----------------------
+// the phased mode polls from the host, so only the persistent solve kernel serves them
+static int check_async(mpcb200_handle* h, unsigned flags, unsigned known)
+{
+    if (h->solve_mode == 1)
+        return set_err(h, MPCB200_E_UNSUPPORTED, "the _async entry points need the fused solve kernel: MPCB200_OPT_SOLVE_MODE 1 polls from the host");
+    if (flags & ~known) return set_err(h, MPCB200_E_INVALID, "unknown flags");
+    return 0;
+}
+
+extern "C" int mpcb200_step_batch_async(mpcb200_handle* h, int B, const double* x0, const double* xf, const double* u_prev, double u_prev_dt,
+                                        const mpcb200_obstacles* obst, const mpcb200_viapoints* vp, const double* x_init,
+                                        const unsigned char* reinit, unsigned flags,
+                                        double* u_seq, double* x_seq, double* dt_out, int* status, double* kkt_err, int* iters)
+{
+    int rc = check_batch(h, B);
+    if (rc) return rc;
+    if ((rc = check_async(h, flags, MPCB200_ASYNC_LINE_OBSTACLES))) return rc;
+    CK(cudaSetDevice(h->device));
+    if ((rc = check_device_arrays(h, "step_batch_async", {x0, xf, u_prev, obst ? obst->count : nullptr, obst ? obst->type : nullptr,
+                                                          obst ? obst->params : nullptr, vp ? vp->count : nullptr, vp ? vp->poses : nullptr,
+                                                          x_init, reinit, u_seq, x_seq, dt_out, status, kkt_err, iters})))
+        return rc;
+    if ((rc = load_inputs(h, h->batch, B, x0, xf, u_prev, u_prev_dt, obst, vp, x_init, reinit, Mem::Device, flags))) return rc;
+    h->B = B;
+    if ((rc = launch_solve_async(h, h->batch, B))) return rc;
+    return fetch_outputs(h, h->batch, B, u_seq, x_seq, dt_out, status, kkt_err, iters, Mem::Device);
+}
+
+extern "C" int mpcb200_step_batch_costmap_async(mpcb200_handle* h, int B, const double* x0, const double* xf, const double* u_prev,
+                                                double u_prev_dt, const mpcb200_costmaps* maps, double behind_robot_dist, int max_per_instance,
+                                                const mpcb200_viapoints* vp, const double* x_init, const unsigned char* reinit,
+                                                double* u_seq, double* x_seq, double* dt_out, int* status, double* kkt_err, int* iters,
+                                                int* obst_found)
+{
+    int rc = check_batch(h, B);
+    if (rc) return rc;
+    if (max_per_instance < 1 || max_per_instance > MAX_OBST_LIST) return set_err(h, MPCB200_E_UNSUPPORTED, "step_batch_costmap: 1..2048 obstacles per instance");
+    if ((rc = check_async(h, 0u, 0u))) return rc;
+    if (!maps) return set_err(h, MPCB200_E_INVALID, "costmap_obstacles: B >= 1, maps, poses and output arrays are required");
+    CK(cudaSetDevice(h->device));
+    if ((rc = check_device_arrays(h, "step_batch_costmap_async", {maps->cost, maps->origin, x0, xf, u_prev, vp ? vp->count : nullptr,
+                                                                  vp ? vp->poses : nullptr, x_init, reinit, u_seq, x_seq, dt_out, status,
+                                                                  kkt_err, iters, obst_found})))
+        return rc;
+    IoBuffers& io = h->batch;
+    if ((rc = io_reserve(h, io, io.rows, max_per_instance))) return rc;
+    if ((rc = load_inputs(h, io, B, x0, xf, u_prev, u_prev_dt, nullptr, vp, x_init, reinit, Mem::Device))) return rc;
+    CostmapOut o;
+    if ((rc = costmap_run(h, B, maps, nullptr, io.x0, behind_robot_dist, max_per_instance, io.obst_count, io.obst_type, io.obst, &o, Mem::Device))) return rc;
+    io.in.obst_count = io.obst_count; io.in.obst_max = max_per_instance;   // point obstacles only: no line-obstacle kernel variant needed
+    h->B = B;
+    if ((rc = launch_solve_async(h, io, B))) return rc;
+    if (obst_found) CK(cudaMemcpyAsync(obst_found, o.found, (size_t)B * 4, cudaMemcpyDeviceToDevice, h->stream));
+    return fetch_outputs(h, io, B, u_seq, x_seq, dt_out, status, kkt_err, iters, Mem::Device);
+}
+
+extern "C" int mpcb200_check_feasible_async(mpcb200_handle* h, int B, const mpcb200_costmaps* maps, const double* x_seq, int n_poses,
+                                            const double* footprint_xy, int n_footprint, double inscribed_radius, double circumscribed_radius,
+                                            double min_resolution_angular, int look_ahead_idx, unsigned char* feasible)
+{
+    (void)circumscribed_radius;
+    int n = 0;
+    if (int rc = check_feasible_args(h, B, maps, x_seq, n_poses, footprint_xy, n_footprint, inscribed_radius, min_resolution_angular, feasible, &n)) return rc;
+    CK(cudaSetDevice(h->device));
+    if (int rc = check_device_arrays(h, "check_feasible_async", {maps->cost, maps->origin, x_seq, n_footprint > 0 ? footprint_xy : nullptr, feasible}))
+        return rc;
+    // maps, footprint and trajectories are read in place; x_seq = NULL: the trajectories of the last solve
+    FeasArgs a{maps->size_x, maps->size_y, maps->resolution, maps->cost, maps->origin, x_seq ? x_seq : h->batch.xseq, n, footprint_xy, n_footprint,
+               inscribed_radius, min_resolution_angular, look_ahead_idx};
+    feasible_kernel<<<grid_for(B, WARPS_PER_CTA), WARPS_PER_CTA * 32, 0, h->stream>>>(a, B, feasible);
+    h->stats.launches_total += 1;
+    CK(cudaGetLastError());
+    return MPCB200_OK;
+}
 
 extern "C" int mpcb200_flush_l2(mpcb200_handle* h)
 {
