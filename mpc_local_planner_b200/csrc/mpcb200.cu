@@ -27,6 +27,7 @@
 
 #include "mpc_device.cuh"
 #include "mpc_costmap.cuh"
+#include "mpc_gate.h"
 
 #define WARPS_PER_CTA 4
 #define MAX_IMG_SMEM (227 * 1024 - 2048)  // dynamic shared memory a CTA may request
@@ -189,7 +190,8 @@ struct FusedArgs
     int* queue;              // next instance
     const int* order;        // queue position -> instance (nullptr: identity)
     unsigned long long* counters;
-    unsigned long long* sm_sync;   // [SMs] phase alignment words (nullptr: off)
+    unsigned long long* sm_sync;   // [sm_words * SMS_WORD_STRIDE] phase alignment words, one line per SM (nullptr: off)
+    int sm_words;                  // SMs with a word
     int sm_gates;                  // 3: gates before eval, KKT and line search; 2: before KKT and line search only
     unsigned long long budget_ns;  // time budget of the launch (max_cpu_time), 0: none
     unsigned long long* origin;    // %globaltimer at the start of the launch: the first CTA sets it (zeroed before the launch)
@@ -197,49 +199,27 @@ struct FusedArgs
 // ---- phase alignment of the CTAs that share an SM ---------------------------------------------------------------------------
 // The solve kernel's iteration is ~128 KB of straight fp64 code, several times an SM's instruction cache: CTAs that sit on the
 // same SM in different phases evict each other's code and every warp streams its instructions from the next cache level.
-// The co-resident CTAs therefore enter each phase of the iteration together: one word per SM in global memory -- generation |
-// arrived | members -- is a barrier
-// with changing membership (a CTA is a member while it iterates, not while it sets up or writes back an instance).
-// The generation counts barriers; generation mod 3 is the phase the barrier opens (eval, KKT, line search): a CTA that arrives
-// out of step keeps arriving (and idles) until the generation matches its phase.  Timing only -- no data crosses CTAs.
+// The co-resident CTAs therefore enter each phase of the iteration together, through a barrier per SM with changing membership
+// (mpc_gate.h).  Each SM's word has a 128-byte line of its own, so the CTAs of different SMs never contend for a line.
+// Timing only -- no data crosses CTAs.
 #define SMS_POLL_NS 128   // pause between two polls of the barrier word (the polling thread shares its scheduler with working warps)
-__device__ __forceinline__ unsigned sm_index() { unsigned r; asm volatile("mov.u32 %0, %%smid;" : "=r"(r)); return r; }
-#define SMS_MEMBERS(w_) ((unsigned)((w_) & 0xFFFFull))
-#define SMS_ARRIVED(w_) ((unsigned)(((w_) >> 16) & 0xFFFFull))
-#define SMS_GEN(w_) ((unsigned)((w_) >> 32))
-#define SMS_PACK(g_, a_, m_) (((unsigned long long)(g_) << 32) | ((unsigned long long)(a_) << 16) | (unsigned long long)(m_))
-__device__ __forceinline__ void sms_join(unsigned long long* st) { atomicAdd(st, 1ull); }
-__device__ __forceinline__ void sms_leave(unsigned long long* st)
+#define SMS_WORD_STRIDE 16   // words: one 128-byte line per SM
+struct DevAtomics
 {
-    unsigned long long old = *(volatile unsigned long long*)st, assumed;
-    do
+    typedef unsigned long long Word;
+    static __device__ __forceinline__ Word add(Word* w, Word v) { return atomicAdd(w, v); }
+    static __device__ __forceinline__ Word cas(Word* w, Word expected, Word desired) { return atomicCAS(w, expected, desired); }
+    // relaxed, not acquire: no data crosses CTAs, and on sm_90a an acquire load is followed by an invalidation of the whole L1
+    // (CCTL.IVALL), so every poll would throw away the cached global data of the CTAs that share the SM
+    static __device__ __forceinline__ Word load(Word* w)
     {
-        assumed = old;
-        unsigned m = SMS_MEMBERS(assumed) - 1u, ar = SMS_ARRIVED(assumed), g = SMS_GEN(assumed);
-        if (ar > 0u && ar >= m) { ar = 0u; ++g; }   // the others were waiting for this CTA only
-        old = atomicCAS(st, assumed, SMS_PACK(g, ar, m));
-    } while (old != assumed);
-}
-__device__ __forceinline__ void sms_arrive(unsigned long long* st, unsigned phase, unsigned nph)
-{
-    for (;;)
-    {
-        unsigned long long old = *(volatile unsigned long long*)st, assumed;
-        unsigned g;
-        bool released;
-        do
-        {
-            assumed = old;
-            unsigned m = SMS_MEMBERS(assumed), ar = SMS_ARRIVED(assumed) + 1u;
-            g = SMS_GEN(assumed);
-            released = ar >= m;
-            old = atomicCAS(st, assumed, released ? SMS_PACK(g + 1u, 0u, m) : SMS_PACK(g, ar, m));
-        } while (old != assumed);
-        if (!released)
-            while (SMS_GEN(*(volatile unsigned long long*)st) == g) __nanosleep(SMS_POLL_NS);
-        if (g % nph == phase) return;
+        Word v;
+        asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(w));
+        return v;
     }
-}
+    static __device__ __forceinline__ void pause() { __nanosleep(SMS_POLL_NS); }
+};
+__device__ __forceinline__ unsigned sm_index() { unsigned r; asm volatile("mov.u32 %0, %%smid;" : "=r"(r)); return r; }
 
 // ---- kernel: queue order of a batch = longest first by the iteration counts of the PREVIOUS solve of the same slots ----
 // A batch costs its slowest instance: an instance that needs 100 iterations and is taken from the queue when the first slots free
@@ -300,7 +280,7 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
 {
     extern __shared__ __align__(128) unsigned char dyn_smem[];
     __shared__ CtaShared sh;
-    __shared__ int s_inst, s_valid;
+    __shared__ int s_inst, s_valid, s_solo;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nt = blockDim.x;
     const int N = L.N;
     double* W = reinterpret_cast<double*>(dyn_smem + IMG_HEAD);
@@ -317,6 +297,7 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
             if (deadline < t0 || deadline == NO_DEADLINE) deadline = NO_DEADLINE - 1;   // saturate
         }
         sh.deadline = deadline;
+        s_solo = 0;
     }
     CudaWarp<EXT> ex;
     ex.lane = lane;
@@ -326,7 +307,9 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
     unsigned long long cyc[MPCB200_NUM_PHASES] = {0, 0, 0, 0, 0}, cyc_total = 0, n_kkt = 0, n_sweeps = 0, n_inst = 0;
     const unsigned nph = (unsigned)a.sm_gates;
     unsigned long long gate_cyc = 0;   // waiting at the phase gates (included in the phase that follows the gate)
-    unsigned long long* sms = a.sm_sync ? a.sm_sync + sm_index() : nullptr;
+    unsigned long long* sms = nullptr;
+    // (PTX does not promise %smid < the SM count: a CTA without a word runs without gates)
+    if (a.sm_sync) { const unsigned smid = sm_index(); if (smid < (unsigned)a.sm_words) sms = a.sm_sync + (size_t)smid * SMS_WORD_STRIDE; }
     const int outer = c.outer_iterations > 0 ? c.outer_iterations : 1;
 // Phase clocks: EVERY thread keeps them (thread 0's are reported).  Not `if (tid == 0)`: a thread-0-only block directly in front of
 // warp-collective code (shuffles, votes) made the compiler split the paths of thread 0 and of lanes 1..31 through the KKT phase in
@@ -371,8 +354,17 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
                 }
                 __syncthreads();
                 TICK(MPCB200_PHASE_ASSOCIATE);
-                if (sms) { if (tid == 0) sms_join(sms); __syncthreads(); }
-#define PHASE_GATE(p_) do { if (sms) { if (tid == 0) { const long long g0_ = clock64(); sms_arrive(sms, p_, nph); gate_cyc += (unsigned long long)(clock64() - g0_); } __syncthreads(); } } while (0)
+                if (sms) { if (tid == 0 && !s_solo) gate::join<DevAtomics>(sms); __syncthreads(); }
+// The tail of a launch, once the queue is drained, runs without gates.  With the queue longest first by history (a.order) the
+// instances still running then are the longest ones, started first, and the step ends with the slowest of them: waiting for its
+// SM neighbours at every phase costs it more than their code in its instruction cache (H100, DESIGN.md 4).  In index order the
+// tail holds instances that started late, and it stays aligned; there a CTA leaves only once it is alone on its SM (every CTA of
+// the SM that could still join holds an instance already).  Thread 0 keeps the flag in shared memory: the iteration loop has
+// no register to spare.
+#define PHASE_GATE(p_) do { if (sms) { if (tid == 0 && !s_solo) { const long long g0_ = clock64(); \
+        const bool drained_ = *(volatile const int*)a.queue >= a.total; \
+        if ((gate::arrive<DevAtomics>(sms, p_, nph) == 1u || a.order) && drained_) { gate::leave<DevAtomics>(sms); s_solo = 1; } \
+        gate_cyc += (unsigned long long)(clock64() - g0_); } __syncthreads(); } } while (0)
                 for (;;)
                 {
                     if (nph == 3u) PHASE_GATE(0u);
@@ -391,7 +383,7 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
                     if (ASC(MPCB200_SC_STATUS) >= 0.0) break;   // jammed: given up
                 }
 #undef PHASE_GATE
-                if (sms) { if (tid == 0) sms_leave(sms); __syncthreads(); }
+                if (sms) { if (tid == 0 && !s_solo) gate::leave<DevAtomics>(sms); __syncthreads(); }
                 if (ASC(MPCB200_SC_STATUS) == (double)MPCB200_STATUS_MAX_TIME) break;   // the budget spans the outer iterations
             }
             // a failed solve leaves nothing to warm-start from
@@ -755,7 +747,7 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
         mpcb200_destroy(h);
         return set_err(nullptr, MPCB200_E_CUDA, m);
     }
-    CKC(cudaMalloc(&h->d_nactive, 8)); CKC(cudaMalloc(&h->d_queue, 4)); CKC(cudaMalloc(&h->d_smsync, 1024 * 8)); CKC(cudaMalloc(&h->d_prev_iters, B * 4)); CKC(cudaMalloc(&h->d_prev_status, B * 4)); CKC(cudaMalloc(&h->d_order, B * 4));
+    CKC(cudaMalloc(&h->d_nactive, 8)); CKC(cudaMalloc(&h->d_queue, 4)); CKC(cudaMalloc(&h->d_smsync, (size_t)h->num_sms * SMS_WORD_STRIDE * 8)); CKC(cudaMalloc(&h->d_prev_iters, B * 4)); CKC(cudaMalloc(&h->d_prev_status, B * 4)); CKC(cudaMalloc(&h->d_order, B * 4));
     CKC(cudaMalloc(&h->d_origin, 8));
     CKC(cudaMalloc(&h->d_counters, CNT_BYTES)); CKC(cudaMemsetAsync(h->d_counters, 0, CNT_BYTES, h->stream));
     CKC(allow_smem(kkt_warp_kernel<false>)); CKC(allow_smem(kkt_warp_kernel<true>));
@@ -970,7 +962,7 @@ static int launch_fused(mpcb200_handle* h, const IoBuffers& io, int total, int q
     FusedArgs a;
     a.ws = h->ws; a.in = io.in; a.out = io.out(); a.total = total; a.queue_mode = queue_mode; a.force_cold = force_cold; a.uprev_dt = io.uprev_dt;
     a.img_words = image_words(h, io.in); a.queue = h->d_queue; a.counters = h->d_counters;
-    a.sm_sync = nullptr; a.sm_gates = h->sm_phase_sync == 2 ? 2 : 3;
+    a.sm_sync = nullptr; a.sm_words = 0; a.sm_gates = h->sm_phase_sync == 2 ? 2 : 3;
     a.order = nullptr;
     a.budget_ns = h->budget_ns; a.origin = h->d_origin;
     if (h->budget_ns) CK(cudaMemsetAsync(h->d_origin, 0, 8, h->stream));
@@ -997,8 +989,8 @@ static int launch_fused(mpcb200_handle* h, const IoBuffers& io, int total, int q
     // phase alignment pays when several CTAs share an SM (auto: from three CTAs per SM)
     if (h->sm_phase_sync > 0 || (h->sm_phase_sync < 0 && per_sm >= 3 && grid > h->num_sms))
     {
-        a.sm_sync = h->d_smsync;
-        CK(cudaMemsetAsync(h->d_smsync, 0, 1024 * 8, h->stream));
+        a.sm_sync = h->d_smsync; a.sm_words = h->num_sms;
+        CK(cudaMemsetAsync(h->d_smsync, 0, (size_t)h->num_sms * SMS_WORD_STRIDE * 8, h->stream));
     }
     CK(cudaMemsetAsync(h->d_queue, 0, 4, h->stream));
     kernel<<<grid, threads, smem, h->stream>>>(h->cfg, h->L, a);
