@@ -54,6 +54,15 @@ int emu_field_offset(const Cfg* c, int field, int* cnt)
     return -1;
 }
 
+// the via-point stages of the last association (not a workspace field of the C ABI); returns their number
+int emu_vp_stage(const Cfg* c, const double* W, int* out)
+{
+    WsLayout L;
+    make_layout(c, MAX_OBST, MAX_VP, L);
+    for (int j = 0; j < L.V; ++j) out[j] = (int)W[L.oVPST + j];
+    return L.V;
+}
+
 void emu_scatter(const Cfg* c, double* W, const double* x0, const double* xf, const double* u_prev, int nobst, const int* types,
                  const double* params, int nvp, const double* vp, const double* x_init, int reinit)
 {

@@ -43,6 +43,7 @@ def lib():
         L.emu_outputs.argtypes = [cp, dp, dp, dp]
         L.emu_resample.argtypes = [C.c_int, dp, dp, C.c_double, C.c_int, dp, dp]
         L.emu_resample.restype = C.c_double
+        L.emu_vp_stage.argtypes = [cp, dp, ip]
         _LIB = L
     return _LIB
 
@@ -107,6 +108,13 @@ class EmuInstance:
             raise ValueError("OBSIDX is written by the association only")
         else:
             self.W[off: off + cnt.value * self.N] = a.reshape(-1)
+
+    def vp_stage(self, n_vp):
+        """the stages the association gave the first n_vp via-points"""
+        out = np.zeros(64, dtype=np.int32)
+        V = self.L.emu_vp_stage(C.byref(self.cfg), _dp(self.W), out.ctypes.data_as(C.POINTER(C.c_int)))
+        assert n_vp <= V
+        return out[:n_vp].copy()
 
     def init(self, force_cold=False):
         self.L.emu_init(C.byref(self.cfg), _dp(self.W), int(force_cold))
