@@ -1,19 +1,11 @@
-"""States of the line-search tests (tests/test_linesearch.py).
-
-A state is the oracle's own interior-point iterate j of one instance (its solve run with max_iter = j), optionally changed at
-the edges of the line search.  Every comparison starts from one such state on both sides, so the two solvers never drift apart.
-"""
+"""States of the line-search tests (tests/test_linesearch.py, tests/test_gpu_linesearch.py): the cases, the iterates and the
+edge changes.  A state is the oracle's own interior-point iterate j of one instance (its solve run with max_iter = j,
+parity.oracle_iterate), optionally changed at the edges of the line search."""
 import numpy as np
 
 from mpc_local_planner_b200 import capi, configs
 
-# the device's own bookkeeping words of SCAL: kept when the oracle's state is written into the device's workspace
-DEVICE_OWN_SCAL = (capi.SC_COLD, capi.SC_VALID, capi.SC_OBST_DROPPED)
-STATE_FIELDS = (("X", capi.F_X), ("U", capi.F_U), ("NU", capi.F_NU), ("S", capi.F_S), ("LAM", capi.F_LAM))
-EVAL_SCAL = (capi.SC_MU, capi.SC_HTT, capi.SC_GT, capi.SC_ERR0, capi.SC_ERRMU, capi.SC_OBJ, capi.SC_INF, capi.SC_BLOG)
 ITERATES = (0, 1, 3, 10, 25, "last")
-# a decision (Armijo test, bin of a blocking ratio) closer than this to its threshold may go either way between two codes
-DECISION_MARGIN = 1e-9
 
 
 def _cfg2_variant(**kw):
@@ -81,47 +73,6 @@ def case(name, n=None):
     return cfg, make_data(b + 1, n), b
 
 
-def is_midpoint(cfg):
-    return cfg.collocation == capi.COLLOC_MIDPOINT
-
-
-def oracle_init(orc, cfg, data, b):
-    o = orc.instance_from_batch(cfg, data, b)
-    o.init_cold(); o.associate()
-    o.L.orc_project_init(orc.C.byref(o.p), o.ws); o.L.orc_init_controls(orc.C.byref(o.p), o.ws)
-    o.init_duals()
-    return o
-
-
-def oracle_iterate(orc, cfg, data, b, j):
-    """The oracle's iterate j (its own solve, stopped by max_iter = j), or the last iterate before convergence (j = "last").
-    Returns the instance, ready for eval(), and whether the solve converged before iterate j."""
-    if j == "last":
-        o = oracle_init(orc, cfg, data, b)
-        r = o.solve()
-        j = max(int(r.iters) - 1, 0)
-    o = oracle_init(orc, cfg, data, b)
-    o.cfg.max_iter = j
-    r = o.solve()
-    o.cfg.max_iter = cfg.max_iter
-    o.arr("SCAL")[capi.SC_STATUS] = -1.0
-    return o, r.status == capi.STATUS_CONVERGED
-
-
-def merged_scal(device_scal, oracle_scal):
-    """the oracle's solver scalars with the device's own bookkeeping words"""
-    s = np.array(oracle_scal, dtype=np.float64, copy=True)
-    for i in DEVICE_OWN_SCAL:
-        s[i] = device_scal[i]
-    return s
-
-
-def step_rows(cfg):
-    """STEP rows that the KKT phase and the oracle's Newton step share: with midpoint differences the heading multiplier row
-    becomes nu+ only in the line search (ls_stage_midpoint_fix), in the oracle at the end of its Newton step"""
-    return 7 if is_midpoint(cfg) else 8
-
-
 # ---- edge states: applied to the oracle's state, then written into the device's -----------------------------------------
 def scale_step(f):
     def mod(o):
@@ -179,20 +130,6 @@ EDGES = {
 }
 
 
-def near_threshold(d):
-    """the oracle's diagnostics show a discrete decision within DECISION_MARGIN of its threshold: a blocking ratio's
-    -2 log2(r) that close to a bin boundary, or a trial's merit that close (relative to the change of the merit it tests)
-    to the Armijo or flat-merit bound.  The merit itself is a sum of terms of the size of phi0 that two codes round
-    differently, by about 1e-13 phi0 measured: that much is added to the margin."""
-    if len(d["phi"]) == 0:   # a null step or a stopped instance: no decision taken
-        return False
-    rnd = 1e-12 * (1.0 + abs(d["phi0"]))
-    armijo = any(abs(p - a) <= DECISION_MARGIN * abs(p - d["phi0"]) + rnd for p, a in zip(d["phi"], d["armijo"]))
-    flat_bound = 1e-13 * (1.0 + abs(d["phi0"]))
-    flat = any(abs(abs(p - d["phi0"]) - flat_bound) <= DECISION_MARGIN * flat_bound + rnd for p in d["phi"][1:])
-    return armijo or flat or d["bin_margin"] <= DECISION_MARGIN
-
-
 def check_edge(name, d, before, after):
     """what each edge state must show in the oracle's diagnostics and scalars (before / after: SCAL around the line search)"""
     if name == "saturated":
@@ -214,53 +151,3 @@ def check_edge(name, d, before, after):
                 assert after[i] == before[i] or (np.isnan(after[i]) and np.isnan(before[i])), i
     elif name == "stopped":
         np.testing.assert_array_equal(after, before)
-
-
-def row_sensitivity(pre, G, DS, d):
-    """Absolute tolerances (S, LAM per row; rho) for the inputs that each side computes itself at the shared iterate: the row
-    values and gradients (the obstacle rows by each side's EVAL, the linear rows by each side's own arithmetic in the line
-    search).  They differ by rounding, taken as dg = 1e-14 (1 + |g| + |g' dz|) per row.  The line search multiplies that by
-    alpha in the slack, by a_dual lambda / s in the multiplier, and by (mu + 2 lambda |ds|) / s / (0.9 inf1) in rho: near
-    convergence an active row's slack is of the size of mu, and these factors reach 1e8 (measured on the CUDA kernels: LAM
-    1.5e-5, rho 1.3e-4 relative, both on obstacle rows; 1.2e-9 absolute on a control-rate row at k = 0).
-    pre: S, LAM and SCAL before the line search; G, DS: the oracle's row values and slack steps; d: its diagnostics."""
-    S, LAM = pre["S"], pre["LAM"]
-    obst = LAM > 0
-    gdz = -(DS + G + S)
-    dg = np.where(obst, 1e-14 * (1.0 + np.abs(G) + np.abs(gdz)), 0.0)
-    sig = np.where(obst, LAM / np.where(obst, S, 1.0), 0.0)
-    tol_s = d["alpha"] * dg
-    tol_lam = d["a_dual"] * sig * dg
-    inf1 = pre["SCAL"][capi.SC_INF]
-    mu = pre["SCAL"][capi.SC_MU]
-    num = (np.where(obst, mu / np.where(obst, S, 1.0), 0.0) * dg + 2.0 * sig * np.abs(DS) * dg).sum()
-    tol_rho = num / (0.9 * inf1) if inf1 > 1e-14 else 0.0
-    return dict(S=tol_s, LAM=tol_lam, rho=tol_rho)
-
-
-def assert_same_outcome(cfg, d, o_arrs, o_scal, dev_arrs, dev_scal, what, rtol=1e-13, rho_tol=1e-10, sens=None):
-    """The line search of the device code against the oracle's from the same inputs.  The discrete outcomes must be equal;
-    a different decision is excused only when the oracle's diagnostics put it within DECISION_MARGIN of its threshold, and
-    then nothing else is compared (returns True).  When both sides decided alike, everything is compared (returns False).
-    sens: row_sensitivity, for the inputs that each side computes itself."""
-    same = all(dev_scal[i] == o_scal[i] for i in (capi.SC_NBT, capi.SC_ITER, capi.SC_TINY, capi.SC_STATUS))
-    if not same and d is not None and near_threshold(d):
-        return True
-    for i in (capi.SC_NBT, capi.SC_ITER, capi.SC_TINY, capi.SC_STATUS):
-        assert dev_scal[i] == o_scal[i], f"{what}: SCAL[{i}] {dev_scal[i]} vs oracle {o_scal[i]}"
-    # rho = (dJ + dphi_bar + curv / 2) / (0.9 inf1) + 1: sums over the rows and stages, accumulated in another order, whose
-    # terms cancel and whose quotient by a small inf1 near convergence magnifies that rounding (up to 1e-12 measured)
-    for i, tol, extra in ((capi.SC_DT, rtol, 0.0), (capi.SC_ALPHA, rtol, 0.0),
-                          (capi.SC_RHO, rho_tol, sens["rho"] if sens else 0.0)):
-        assert abs(dev_scal[i] - o_scal[i]) <= tol * abs(o_scal[i]) + extra, \
-            f"{what}: SCAL[{i}] {dev_scal[i]!r} vs oracle {o_scal[i]!r}"
-    for nm, _ in STATE_FIELDS:
-        a, b = dev_arrs[nm], o_arrs[nm]
-        # with midpoint differences the heading multiplier row of the step is the device's own (see step_rows), so NU agrees
-        # to the tolerance of the Newton step only
-        tol = 1e-7 if nm == "NU" and is_midpoint(cfg) else rtol
-        bound = tol * max(1.0, np.abs(b).max()) + (sens[nm] if sens and nm in sens else 0.0)
-        excess = np.abs(a - b) - bound
-        assert (excess <= 0).all(), \
-            f"{what}: {nm} differs by {np.abs(a - b).max():.3e}, worst at {np.unravel_index(np.argmax(excess), a.shape)}"
-    return False

@@ -18,10 +18,7 @@ import numpy as np
 
 import linesearch_cases as lc
 from mpc_local_planner_b200 import capi, configs
-
-UNI_QF = (capi.MODEL_UNI_POINT, capi.PROBLEM_FIXED_DT_QF)
-UNI = (capi.MODEL_UNI_POINT, capi.PROBLEM_GENERIC)
-GEN = (capi.MODEL_GENERIC, capi.PROBLEM_GENERIC)
+from parity import GEN, UNI, UNI_QF
 
 
 # ---- robot models (the bounds of test_gpu_variants.test_robot_models) ----

@@ -4,8 +4,7 @@ tests/test_gpu_parity.py on the GPU."""
 import numpy as np
 import pytest
 
-import linesearch_cases as lc
-import test_linesearch as tls
+import parity as par
 from mpc_local_planner_b200 import capi, configs
 
 
@@ -13,53 +12,19 @@ def _data(cid, B):
     return configs.g1_instance() if cid == 1 else configs.generate(cid, B)
 
 
-def _oracle_init(orc, cfg, data, b):
-    o = orc.instance_from_batch(cfg, data, b)
-    o.init_cold(); o.associate()
-    o.L.orc_project_init(orc.C.byref(o.p), o.ws); o.L.orc_init_controls(orc.C.byref(o.p), o.ws)
-    o.init_duals()
-    return o
-
-
 @pytest.mark.parametrize("cid,b", [(1, 0), (2, 0), (2, 2), (3, 2), (4, 1)])
 def test_phases_match_oracle(orc, emu, cid, b):
     cfg = configs.config_for(cid, tol=1e-8)
     data = _data(cid, b + 1)
-    o = _oracle_init(orc, cfg, data, b)
+    o = par.oracle_init(orc, cfg, data, b)
     e = emu.instance_from_batch(cfg, data, b)
     e.init(); e.associate()
-    np.testing.assert_allclose(e.field(capi.F_X), o.arr("X"), atol=1e-13)
-    np.testing.assert_allclose(e.field(capi.F_U), o.arr("U"), atol=1e-13)
-    np.testing.assert_array_equal(e.field(capi.F_OBSIDX), o.arr("OBSIDX"))
-    np.testing.assert_allclose(e.field(capi.F_S), o.arr("S"), rtol=1e-9)
-    np.testing.assert_allclose(e.field(capi.F_LAM), o.arr("LAM"), rtol=1e-9)
-    idx = [capi.SC_DT, capi.SC_MU, capi.SC_HTT, capi.SC_GT, capi.SC_ERR0, capi.SC_ERRMU, capi.SC_OBJ, capi.SC_INF, capi.SC_BLOG]
+    par.assert_init(*par.emu_init_fields(e), o, par.EMU)
+    steps = marginal = 0
     for it in range(4):
-        o.eval(); e.eval()
-        scale = np.abs(o.arr("KKT")).max()
-        np.testing.assert_allclose(e.field(capi.F_KKT), o.arr("KKT"), atol=1e-9 * scale)
-        np.testing.assert_allclose(e.field(capi.F_SCAL)[idx], o.arr("SCAL")[idx], rtol=1e-8, atol=1e-10)
-        assert e.kkt() == 0
-        # the emulator's regularisation bookkeeping is the one both sides continue with
-        for i in (capi.SC_DELTA_LAST, capi.SC_NREG):
-            o.arr("SCAL")[i] = e.field(capi.F_SCAL)[i]
-        if e.field(capi.F_SCAL)[capi.SC_DEFER] != 0.0:
-            # factorisation budget spent: null step, the escalation resumes at DELTA_LAST / 3 in the next iteration
-            nxt = e.field(capi.F_SCAL)[capi.SC_DELTA_LAST] / 3.0
-            assert o.kkt_solve(nxt / 8.0) == 1 or o.kkt_solve(nxt / 100.0) == 1
-            o.arr("SCAL")[capi.SC_DEFER] = 1.0
-        else:
-            delta = e.field(capi.F_SCAL)[capi.SC_DELTA]
-            assert o.kkt_solve(delta) == 0
-            sscale = max(np.abs(o.arr("STEP")).max(), 1.0)
-            np.testing.assert_allclose(e.field(capi.F_STEP), o.arr("STEP"), atol=1e-7 * sscale)
-            assert e.field(capi.F_SCAL)[capi.SC_DDT] == pytest.approx(o.arr("SCAL")[capi.SC_DDT], abs=1e-9 * max(1, abs(o.arr("SCAL")[capi.SC_DDT])))
-        # one line search on each side from the oracle's records, step and scalars, compared (tests/test_linesearch.py); the
-        # oracle's iterate is then the shared state of the next iteration
-        tls.run_both(o, e, cfg, f"cfg {cid}, iteration {it}")
-        for name, f in lc.STATE_FIELDS:
-            e.set_field(f, o.arr(name))
-        e.set_field(capi.F_SCAL, lc.merged_scal(e.field(capi.F_SCAL), o.arr("SCAL")))
+        s, m = par.emu_iterate(o, e, cfg, f"cfg {cid}, iteration {it}")
+        steps += s; marginal += m
+    assert steps >= 1 and marginal <= 1, (steps, marginal)
 
 
 @pytest.mark.parametrize("cid,B", [(1, 1), (2, 16), (3, 8), (4, 8), (5, 12)])
@@ -123,14 +88,11 @@ def test_line_obstacles_match_oracle(orc, emu, cid, B):
     ref = orc.step_batch(cfg, data, n_threads=2)
     agree = 0
     for b in range(B):
-        o = _oracle_init(orc, cfg, data, b)
+        o = par.oracle_init(orc, cfg, data, b)
         e = emu.instance_from_batch(cfg, data, b)
         e.init(); e.associate()
-        np.testing.assert_allclose(e.field(capi.F_X), o.arr("X"), atol=1e-12)
-        np.testing.assert_array_equal(e.field(capi.F_OBSIDX), o.arr("OBSIDX"))
-        o.eval(); e.eval()
-        scale = np.abs(o.arr("KKT")).max()
-        np.testing.assert_allclose(e.field(capi.F_KKT), o.arr("KKT"), atol=1e-9 * scale)
+        par.assert_init(*par.emu_init_fields(e), o, par.EMU)
+        par.emu_assert_eval(o, e)
         st = e.solve()
         u, x = e.outputs()
         agree += st == ref["status"][b]
@@ -151,14 +113,11 @@ def test_integral_form_cost_matches_oracle(orc, emu, rule):
     ref = orc.step_batch(cfg, data, n_threads=2)
     n_both = 0
     for b in range(B):
-        o = _oracle_init(orc, cfg, data, b)
+        o = par.oracle_init(orc, cfg, data, b)
         e = emu.instance_from_batch(cfg, data, b)
         e.init(); e.associate()
-        o.eval(); e.eval()
-        scale = np.abs(o.arr("KKT")).max()
-        np.testing.assert_allclose(e.field(capi.F_KKT), o.arr("KKT"), atol=1e-9 * scale)
-        idx = [capi.SC_HTT, capi.SC_GT, capi.SC_OBJ, capi.SC_ERR0]
-        np.testing.assert_allclose(e.field(capi.F_SCAL)[idx], o.arr("SCAL")[idx], rtol=1e-8, atol=1e-10)
+        par.assert_init(*par.emu_init_fields(e), o, par.EMU)
+        par.emu_assert_eval(o, e)
         st = e.solve()
         u, x = e.outputs()
         if st == 0 and ref["status"][b] == 0:
@@ -177,13 +136,11 @@ def test_terminal_ball_matches_oracle(orc, emu):
     ref = orc.step_batch(cfg, data, n_threads=2)
     n_both = n_active = 0
     for b in range(B):
-        o = _oracle_init(orc, cfg, data, b)
+        o = par.oracle_init(orc, cfg, data, b)
         e = emu.instance_from_batch(cfg, data, b)
         e.init(); e.associate()
-        np.testing.assert_allclose(e.field(capi.F_S), o.arr("S"), rtol=1e-9)
-        o.eval(); e.eval()
-        scale = np.abs(o.arr("KKT")).max()
-        np.testing.assert_allclose(e.field(capi.F_KKT), o.arr("KKT"), atol=1e-9 * scale)
+        par.assert_init(*par.emu_init_fields(e), o, par.EMU)
+        par.emu_assert_eval(o, e)
         st = e.solve()
         u, x = e.outputs()
         if st == 0 and ref["status"][b] == 0:
@@ -208,17 +165,12 @@ def test_dynamic_obstacles_match_oracle(orc, emu, free_dt):
     ref = orc.step_batch(cfg, data, n_threads=2)
     n_both = 0
     for b in range(B):
-        o = _oracle_init(orc, cfg, data, b)
+        o = par.oracle_init(orc, cfg, data, b)
         e = emu.instance_from_batch(cfg, data, b)
         e.init(); e.associate()
-        np.testing.assert_array_equal(e.field(capi.F_OBSIDX), o.arr("OBSIDX"))
+        par.assert_init(*par.emu_init_fields(e), o, par.EMU)
         assert (o.arr("OBSIDX")[:, 1:-1] >= 0).all()  # all (moving) obstacles are kept at every stage
-        np.testing.assert_allclose(e.field(capi.F_X), o.arr("X"), atol=1e-12)
-        o.eval(); e.eval()
-        scale = np.abs(o.arr("KKT")).max()
-        np.testing.assert_allclose(e.field(capi.F_KKT), o.arr("KKT"), atol=1e-9 * scale)
-        idx = [capi.SC_HTT, capi.SC_GT, capi.SC_ERR0]
-        np.testing.assert_allclose(e.field(capi.F_SCAL)[idx], o.arr("SCAL")[idx], rtol=1e-8, atol=1e-10)
+        par.emu_assert_eval(o, e)
         st = e.solve()
         u, x = e.outputs()
         if st == 0 and ref["status"][b] == 0:
@@ -254,14 +206,11 @@ def test_midpoint_differences_match_oracle(orc, emu, base):
     n_both = 0
     n_other_optimum = 0
     for b in range(B):
-        o = _oracle_init(orc, cfg, data, b)
+        o = par.oracle_init(orc, cfg, data, b)
         e = emu.instance_from_batch(cfg, data, b)
         e.init(); e.associate()
-        o.eval(); e.eval()
-        scale = np.abs(o.arr("KKT")).max()
-        np.testing.assert_allclose(e.field(capi.F_KKT), o.arr("KKT"), atol=1e-9 * scale)
-        idx = [capi.SC_HTT, capi.SC_GT, capi.SC_OBJ, capi.SC_ERR0]
-        np.testing.assert_allclose(e.field(capi.F_SCAL)[idx], o.arr("SCAL")[idx], rtol=1e-8, atol=1e-10)
+        par.assert_init(*par.emu_init_fields(e), o, par.EMU)
+        par.emu_assert_eval(o, e)
         st = e.solve()
         u, x = e.outputs()
         if st == 0 and ref["status"][b] == 0:

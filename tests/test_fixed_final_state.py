@@ -9,90 +9,11 @@ no d(dt) unknown (fixed dt, some component fixed); the terminal cost and ball be
 import numpy as np
 import pytest
 
+import dense_kkt as dk
 import golden_checks as gc
-import linesearch_cases as lc
-import test_linesearch as tls
-import test_oracle_functions as tof
-from mpc_local_planner_b200 import capi, configs
-
-
-def _stack(a, b):
-    """one batch of the instances of a, then those of b (obstacle lists padded to the longer one)"""
-    ca, ta, pa = a["obstacles"]; cb, tb, pb = b["obstacles"]
-    M = max(ta.shape[1], tb.shape[1])
-    pad_t = lambda t: np.pad(t, ((0, 0), (0, M - t.shape[1])))
-    pad_p = lambda p: np.pad(p, ((0, 0), (0, M - p.shape[1]), (0, 0)))
-    return dict(x0=np.concatenate([a["x0"], b["x0"]]), xf=np.concatenate([a["xf"], b["xf"]]),
-                u_prev=np.concatenate([a["u_prev"], b["u_prev"]]), u_prev_dt=b["u_prev_dt"],
-                obstacles=(np.concatenate([ca, cb]).astype(np.int32), np.concatenate([pad_t(ta), pad_t(tb)]),
-                           np.concatenate([pad_p(pa), pad_p(pb)])), viapoints=None)
-
-
-def _g1_then_generated(B):
-    """G1 (the reference's own scenario) first, then cfg-2 style instances at N = 20"""
-    g1 = configs.g1_instance()
-    if B == 1:
-        return g1
-    gen = configs.generate(5, B - 1, n=20)
-    g1["u_prev_dt"] = gen["u_prev_dt"]
-    return _stack(g1, gen)
-
-
-def _with_mask(make, mask, **kw):
-    def f():
-        c = make(tol=1e-8, **kw)
-        c.xf_fixed[:] = mask
-        # a fixed goal with a fixed dt: the reference's cold guess (zero controls) leaves the linearised fixed-goal rows rank
-        # deficient (see tests/golden/golden_cases.py); start from the solver's seeded guess
-        if not c.variable_dt:
-            c.reference_initial_guess = 0
-        return c
-    return f
-
-
-def _midpoint_integral(tol):
-    c = configs.cfg2_integral_form(tol=tol)
-    c.collocation = capi.COLLOC_MIDPOINT
-    return c
-
-
-# Fixed-dt fixed-goal cases run on cfg-2 style instances with goals 2.1 - 4.2 m away (generate(5, ., n=35)), all reachable in
-# 14.7 s.  Reachability is not what limits convergence here: closer goals (more spare time) converge LESS often, and with the
-# whole goal pose fixed the oracle converges on 18 of the first 48.  The cause is not established; the interior-point method
-# here has no constraint regularisation (Ipopt's delta_c).
-_QF_DATA = lambda B: configs.generate(5, B, n=35)
-# name -> (configuration, data(B))
-FIXED_CASES = {
-    "mt_heading_free": (_with_mask(configs.cfg1, [1, 1, 0]), _g1_then_generated),
-    "mt_x_only": (_with_mask(configs.cfg1, [1, 0, 0]), _g1_then_generated),
-    "qf_goal_fixed": (_with_mask(configs.cfg2, [1, 1, 1]), _QF_DATA),
-    "qf_position_fixed": (_with_mask(configs.cfg2, [1, 1, 0]), _QF_DATA),
-    "qf_heading_fixed": (_with_mask(configs.cfg2, [0, 0, 1]), _QF_DATA),
-    "trap_position_fixed": (_with_mask(configs.cfg2_trapezoidal, [1, 1, 0], variable_dt=True), lambda B: configs.generate(2, B)),
-    "midpoint_position_fixed": (_with_mask(_midpoint_integral, [1, 1, 0]), lambda B: configs.generate(2, B)),
-    "ball_y_fixed": (_with_mask(configs.cfg2_terminal_ball, [0, 1, 0]), lambda B: configs.generate(2, B)),
-    "car_heading_free": (_with_mask(configs.cfg3, [1, 1, 0], n=80), lambda B: configs.generate(3, B)),
-}
-SHIPPED = {
-    "cfg1": (lambda: configs.cfg1(tol=1e-8), _g1_then_generated),
-    "cfg3": (lambda: configs.cfg3(tol=1e-8), lambda B: configs.generate(3, B)),
-}
-
-
-def case(name):
-    make_cfg, make_data = {**FIXED_CASES, **SHIPPED}[name]
-    return make_cfg(), make_data
-
-
-def fixed_components(cfg):
-    return [i for i in range(3) if cfg.xf_fixed[i]]
-
-
-def assert_fixed_components_exact(cfg, x_last, xf, what):
-    """every fixed component of the final state equals the goal bit for bit (headings of the goals lie in [-pi, pi), where the
-    output normalisation is the identity)"""
-    for i in fixed_components(cfg):
-        assert x_last[i] == xf[i], f"{what}: x_(N-1),{i} - xf_{i} = {x_last[i] - xf[i]:.3e}"
+import parity as par
+from fixed_cases import FIXED_CASES, GOLDEN_CASES, SHIPPED, assert_fixed_components_exact, case, moved_goal
+from mpc_local_planner_b200 import capi
 
 
 def assert_same_status(cfg, st_a, it_a, st_b, it_b, what):
@@ -104,20 +25,6 @@ def assert_same_status(cfg, st_a, it_a, st_b, it_b, what):
     assert marginal, f"{what}: status {st_a} ({it_a} iterations) vs {st_b} ({it_b} iterations)"
 
 
-def moved_goal(xf):
-    g = np.array(xf, dtype=np.float64).copy()
-    g[0] += 0.2; g[1] -= 0.2; g[2] = g[2] + 0.1 if g[2] + 0.1 < np.pi else g[2] - 0.1
-    return g
-
-
-def _oracle_init(orc, cfg, data, b):
-    o = orc.instance_from_batch(cfg, data, b)
-    o.init_cold(); o.associate()
-    o.L.orc_project_init(orc.C.byref(o.p), o.ws); o.L.orc_init_controls(orc.C.byref(o.p), o.ws)
-    o.init_duals()
-    return o
-
-
 # ---- the oracle's Newton step against the dense KKT system ----
 @pytest.mark.parametrize("name", list(FIXED_CASES))
 def test_newton_step_matches_dense_kkt(orc, name):
@@ -127,9 +34,9 @@ def test_newton_step_matches_dense_kkt(orc, name):
     data = make_data(2)
     compared = 0
     for nu_scale in (1.0, 0.05):
-        compared += tof._check_gradient_and_newton_step(orc, None, nu_scale, cfg=cfg, data=data, b=0)
+        compared += dk.check_gradient_and_newton_step(orc, None, nu_scale, cfg=cfg, data=data, b=0)
     if compared == 0:   # every regularisation hit the conservative pivot test on this iterate: another instance and seed
-        compared += tof._check_gradient_and_newton_step(orc, None, 0.05, cfg=cfg, data=data, b=1, seed=1)
+        compared += dk.check_gradient_and_newton_step(orc, None, 0.05, cfg=cfg, data=data, b=1, seed=1)
     assert compared >= 1
 
 
@@ -141,54 +48,15 @@ def test_phases_match_oracle(orc, emu, name):
     cfg, make_data = case(name)
     b = 1
     data = make_data(b + 1)
-    o = _oracle_init(orc, cfg, data, b)
+    o = par.oracle_init(orc, cfg, data, b)
     e = emu.instance_from_batch(cfg, data, b)
     e.init(); e.associate()
-    np.testing.assert_allclose(e.field(capi.F_X), o.arr("X"), atol=1e-13)
-    np.testing.assert_allclose(e.field(capi.F_U), o.arr("U"), atol=1e-13)
-    np.testing.assert_array_equal(e.field(capi.F_OBSIDX), o.arr("OBSIDX"))
-    np.testing.assert_allclose(e.field(capi.F_S), o.arr("S"), rtol=1e-9)
-    np.testing.assert_allclose(e.field(capi.F_LAM), o.arr("LAM"), rtol=1e-9)
-    idx = [capi.SC_DT, capi.SC_MU, capi.SC_HTT, capi.SC_GT, capi.SC_ERR0, capi.SC_ERRMU, capi.SC_OBJ, capi.SC_INF, capi.SC_BLOG]
-    n_steps = 0
+    par.assert_init(*par.emu_init_fields(e), o, par.EMU)
+    steps = marginal = 0
     for it in range(4):
-        o.eval(); e.eval()
-        np.testing.assert_array_equal(e.field(capi.F_OBSIDX), o.arr("OBSIDX"))
-        scale = np.abs(o.arr("KKT")).max()
-        np.testing.assert_allclose(e.field(capi.F_KKT), o.arr("KKT"), atol=1e-9 * scale)
-        np.testing.assert_allclose(e.field(capi.F_SCAL)[idx], o.arr("SCAL")[idx], rtol=1e-8, atol=1e-10)
-        assert e.kkt() == 0
-        for i in (capi.SC_DELTA_LAST, capi.SC_NREG):   # the emulator's regularisation bookkeeping is the one both continue with
-            o.arr("SCAL")[i] = e.field(capi.F_SCAL)[i]
-        if e.field(capi.F_SCAL)[capi.SC_DEFER] != 0.0:
-            nxt = e.field(capi.F_SCAL)[capi.SC_DELTA_LAST] / 3.0
-            assert o.kkt_solve(nxt / 8.0) == 1 or o.kkt_solve(nxt / 100.0) == 1
-            o.arr("SCAL")[capi.SC_DEFER] = 1.0
-            tls.run_both(o, e, cfg, f"{name}, iteration {it} (null step)")
-        else:
-            delta = e.field(capi.F_SCAL)[capi.SC_DELTA]
-            assert o.kkt_solve(delta) == 0
-            STEP = e.field(capi.F_STEP)
-            sscale = max(np.abs(o.arr("STEP")).max(), 1.0)
-            # midpoint differences: the device turns the heading multiplier of the condensed system into nu+ at the start of
-            # the line search (ls_stage_midpoint_fix), the oracle at the end of its solve; that row is compared after it
-            rows = 7 if cfg.collocation == capi.COLLOC_MIDPOINT else 8
-            np.testing.assert_allclose(STEP[:rows], o.arr("STEP")[:rows], atol=1e-7 * sscale)
-            for i in fixed_components(cfg):   # a fixed component is not a variable: no step at all
-                assert STEP[i, -1] == 0.0 and o.arr("STEP")[i, -1] == 0.0
-            ddt_o = o.arr("SCAL")[capi.SC_DDT]
-            assert e.field(capi.F_SCAL)[capi.SC_DDT] == pytest.approx(ddt_o, abs=1e-9 * max(1, abs(ddt_o)))
-            if not cfg.variable_dt:
-                assert e.field(capi.F_SCAL)[capi.SC_DDT] == 0.0 and ddt_o == 0.0
-            n_steps += 1
-            # one line search on each side from the oracle's records, step and scalars, compared (tests/test_linesearch.py)
-            tls.run_both(o, e, cfg, f"{name}, iteration {it}")
-            np.testing.assert_allclose(e.field(capi.F_STEP)[rows:], o.arr("STEP")[rows:], atol=1e-7 * sscale)
-        # the oracle's iterate is the shared state of the next iteration
-        for nm, f in lc.STATE_FIELDS:
-            e.set_field(f, o.arr(nm))
-        e.set_field(capi.F_SCAL, lc.merged_scal(e.field(capi.F_SCAL), o.arr("SCAL")))
-    assert n_steps >= 1
+        s, m = par.emu_iterate(o, e, cfg, f"{name}, iteration {it}")
+        steps += s; marginal += m
+    assert steps >= 1 and marginal <= 1, (steps, marginal)
 
 
 def _emu_solves(emu, cfg, data, B):
@@ -287,11 +155,6 @@ def test_fixed_components_stay_exactly_at_the_goal(orc, emu, name):
 
 
 # ---- golden fixtures (SLSQP on the independent numpy restatement) ----
-# With a fixed dt and a fixed goal position the interior-point method fails (maximum iterations or numerical error) on instances
-# where SLSQP finds a feasible optimum; expected to fail until that is fixed.
-_NOT_SOLVED = pytest.mark.xfail(strict=True, reason="fixed dt + fixed goal position: the interior-point solve does not converge "
-                                                     "on most instances SLSQP solves")
-GOLDEN_CASES = ["g1_heading_free", pytest.param("cfg2_goal_fixed", marks=_NOT_SOLVED), pytest.param("cfg2_position_fixed", marks=_NOT_SOLVED)]
 @pytest.mark.parametrize("gcase", GOLDEN_CASES)
 def test_golden_cases(orc, gcase):
     matched, other = gc.check_case(gcase, lambda cfg, data: orc.step_batch(cfg, data, n_threads=4))

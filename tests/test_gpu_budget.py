@@ -9,6 +9,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import costmap_cases as cm
 from mpc_local_planner_b200 import capi, configs
 from tests.conftest import ROOT
 
@@ -86,7 +87,6 @@ def test_no_budget_changes_nothing(cuda_lib, case):
 
 
 def test_no_budget_changes_nothing_in_the_queue_and_the_costmap_cycle(cuda_lib):
-    from test_gpu_variants import _costmap_scene
     cfg = configs.cfg2(tol=1e-6)
     data = configs.generate(2, 1536)
     res = {}
@@ -96,7 +96,7 @@ def test_no_budget_changes_nothing_in_the_queue_and_the_costmap_cycle(cuda_lib):
         s.close()
     _assert_same(res[-1.0], res[None]); _assert_same(res[1e6], res[None])
     B, M = 32, 512
-    cost, origin, r, pose, goal = _costmap_scene(B, 0.006, 11)
+    cost, origin, r, pose, goal = cm.costmap_scene(B, 0.006, 11)
     for t in (None, -1.0, 1e6):
         s = capi.BatchSolver(cfg if t is None else _with_budget(cfg, t), B, device=0)
         res[t] = s.step_from_costmaps(pose, goal, cost, origin, r, 0.3, M, u_prev=np.zeros((B, 2)), u_prev_dt=0.2)

@@ -6,6 +6,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import costmap_cases as cm
 from mpc_local_planner_b200 import capi, configs
 
 pytestmark = pytest.mark.gpu
@@ -50,9 +51,8 @@ def _step_async(s, x0, xf, u_prev, u_prev_dt, obst, vp, **kw):
 
 
 def _long_list_case(B):
-    from test_gpu_variants import _costmap_scene
     M = 250
-    cost, origin, res, pose, goal = _costmap_scene(B, 0.006, 11)
+    cost, origin, res, pose, goal = cm.costmap_scene(B, 0.006, 11)
     s = capi.BatchSolver(configs.cfg2(), B, device=0)
     (count, typ, par), _ = s.costmap_obstacles(cost, origin, res, pose, 0.3, M)
     s.close()
@@ -152,10 +152,9 @@ def test_mixed_sequence_shares_the_batch_state(cuda_lib):
 
 
 def _scene(B, W, H, seed):
-    from test_oracle_functions import _random_costmap
     rng = np.random.default_rng(seed)
     res = 0.05
-    cost = np.stack([_random_costmap(rng, W, H, 0.006) for _ in range(B)])
+    cost = np.stack([cm.random_costmap(rng, W, H, 0.006) for _ in range(B)])
     origin = rng.uniform(-3, 3, (B, 2))
     pose = np.concatenate([origin + rng.uniform(2.5, 4.0, (B, 2)), rng.uniform(-np.pi, np.pi, (B, 1))], axis=1)
     goal = pose.copy(); goal[:, 0] += 3.0 * np.cos(pose[:, 2]); goal[:, 1] += 3.0 * np.sin(pose[:, 2])
@@ -202,11 +201,10 @@ def test_costmap_chain_async_equals_blocking(cuda_lib, W, offset):
 
 @pytest.mark.parametrize("footprint", ["polygon", "two_points"])
 def test_check_feasible_async_equals_blocking(cuda_lib, footprint):
-    from tests.test_oracle_functions import _feasibility_cases
     rng = np.random.default_rng(5)
     fp = np.array(configs.CARLIKE_POLYGON) if footprint == "polygon" else np.array([[0.1, 0.0], [-0.1, 0.0]])
     B = 96
-    cases = _feasibility_cases(rng, B)
+    cases = cm.feasibility_cases(rng, B)
     cost = np.stack([c[0] for c in cases]); origin = np.stack([c[1] for c in cases]); xs = np.stack([c[2] for c in cases])
     cfg = configs.cfg2()
     st = torch.cuda.Stream()

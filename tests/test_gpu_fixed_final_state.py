@@ -1,23 +1,17 @@
 """grid/xf_fixed component by component on the CUDA kernels (the cases of tests/test_fixed_final_state.py): phase parity at the
-first iterate, whole solves through the C ABI in both solve modes, the specialised unicycle / point kernels with a fixed dt and a
-fixed goal against the generic ones, the golden fixtures, and fixed components that stay exactly at the goal."""
+first iterate, whole solves through the C ABI in both solve modes, the golden fixtures, and fixed components that stay exactly at
+the goal.  The specialised unicycle / point kernels with a fixed dt and a fixed goal are compared with the generic ones in
+tests/test_gpu_kernel_keys.py."""
 import numpy as np
 import pytest
 
 import golden_checks as gc
+import parity as par
+from fixed_cases import FIXED_CASES, GOLDEN_CASES, SHIPPED, assert_fixed_components_exact, case, moved_goal
 from mpc_local_planner_b200 import capi, configs
-from test_fixed_final_state import FIXED_CASES, GOLDEN_CASES, SHIPPED, assert_fixed_components_exact, case, fixed_components, moved_goal
 
 pytestmark = pytest.mark.gpu
 U_TOL = 1e-4
-
-
-def _oracle_init(orc, cfg, data, b):
-    o = orc.instance_from_batch(cfg, data, b)
-    o.init_cold(); o.associate()
-    o.L.orc_project_init(orc.C.byref(o.p), o.ws); o.L.orc_init_controls(orc.C.byref(o.p), o.ws)
-    o.init_duals()
-    return o
 
 
 def _step(s, data, x0=None, xf=None, u_prev=None, u_prev_dt=None):
@@ -32,43 +26,7 @@ def test_phase_parity(cuda_lib, orc, name):
     cfg, make_data = case(name)
     B = 6
     data = make_data(B)
-    s = capi.BatchSolver(cfg, B, device=0)
-    s.upload(data["x0"], data["xf"], data["u_prev"], data["u_prev_dt"], data["obstacles"], data["viapoints"])
-    s.run_phase(capi.PHASE_INIT); s.run_phase(capi.PHASE_ASSOCIATE)
-    X, U, S, LAM, OBS = (s.ws_read(f) for f in (capi.F_X, capi.F_U, capi.F_S, capi.F_LAM, capi.F_OBSIDX))
-    s.run_phase(capi.PHASE_EVAL)
-    KKT, SC = s.ws_read(capi.F_KKT), s.ws_read(capi.F_SCAL)
-    s.run_phase(capi.PHASE_KKT)
-    STEP, SC2 = s.ws_read(capi.F_STEP), s.ws_read(capi.F_SCAL)
-    s.close()
-    n_steps = 0
-    for b in range(B):
-        o = _oracle_init(orc, cfg, data, b)
-        np.testing.assert_allclose(X[b], o.arr("X"), rtol=0, atol=1e-12)
-        np.testing.assert_allclose(U[b], o.arr("U"), rtol=0, atol=1e-12)
-        np.testing.assert_array_equal(OBS[b], o.arr("OBSIDX"))
-        np.testing.assert_allclose(S[b], o.arr("S"), rtol=1e-11, atol=1e-13)
-        np.testing.assert_allclose(LAM[b], o.arr("LAM"), rtol=1e-10, atol=1e-13)
-        o.eval()
-        scale = np.abs(o.arr("KKT")).max()
-        np.testing.assert_allclose(KKT[b], o.arr("KKT"), rtol=0, atol=1e-11 * scale)
-        idx = [capi.SC_MU, capi.SC_HTT, capi.SC_GT, capi.SC_ERR0, capi.SC_ERRMU, capi.SC_OBJ, capi.SC_INF, capi.SC_BLOG]
-        np.testing.assert_allclose(SC[b][idx], o.arr("SCAL")[idx], rtol=1e-10, atol=1e-12)
-        if SC2[b][capi.SC_DEFER] != 0.0:
-            assert o.kkt_solve(0.0) == 1   # factorisation budget spent at this iterate: wrong inertia at delta = 0 for both
-            continue
-        delta = SC2[b][capi.SC_DELTA]
-        if delta != 0.0:
-            assert o.kkt_solve(0.0) == 1   # both see the wrong inertia at delta = 0; the regularised steps are compared
-        assert o.kkt_solve(delta) == 0
-        sscale = np.abs(o.arr("STEP")).max()
-        # (midpoint differences: the heading multiplier row is finished at the start of the line search, see the CPU test)
-        rows = 7 if cfg.collocation == capi.COLLOC_MIDPOINT else 8
-        np.testing.assert_allclose(STEP[b][:rows], o.arr("STEP")[:rows], rtol=0, atol=1e-9 * sscale)
-        for i in fixed_components(cfg):
-            assert STEP[b][i, -1] == 0.0
-        assert abs(SC2[b][capi.SC_DDT] - o.arr("SCAL")[capi.SC_DDT]) <= 1e-9 * max(1.0, abs(o.arr("SCAL")[capi.SC_DDT]))
-        n_steps += 1
+    n_steps = par.check_first_iterate(orc, cfg, data, B)
     # the car's cold start needs more regularisation than one iteration's factorisation budget on every instance (its steps are
     # compared over four iterations on the emulator, tests/test_fixed_final_state.py)
     assert n_steps >= (0 if name == "car_heading_free" else 1)
@@ -108,43 +66,6 @@ def test_solve_parity(cuda_lib, orc, name, n, B, mode):
     assert (out["kkt_err"][both] <= cfg.tol).all()
     for b in range(B):   # converged or not
         assert_fixed_components_exact(cfg, out["x_seq"][b, -1], data["xf"][b], f"{name} instance {b} (status {out['status'][b]})")
-
-
-FIELDS = ("status", "iters", "u_seq", "x_seq", "dt", "kkt_err")
-
-
-def _bits(a):
-    a = np.ascontiguousarray(a)
-    return a.view(np.uint64) if a.dtype == np.float64 else a
-
-
-def _solve_twice(cfg, data, B, force_generic):
-    s = capi.BatchSolver(cfg, B, device=0)
-    s.set_option(capi.OPT_FORCE_GENERIC_MODEL, force_generic)
-    outs = []
-    for _ in range(2):   # cold, then warm from the first solve
-        out = _step(s, data)
-        outs.append({f: np.array(out[f], copy=True) for f in FIELDS})
-    keys = (s.kernel_model(), s.kernel_problem())
-    s.close()
-    return outs, keys
-
-
-@pytest.mark.parametrize("name", ["qf_position_fixed", "qf_goal_fixed"])
-def test_specialised_kernels_match_the_generic_ones(cuda_lib, name):
-    """A fixed dt with a fixed goal component runs the unicycle / point kernel of the bordered KKT system with the generic
-    problem code; it computes what the generic kernel computes, bit for bit, cold and warm."""
-    cfg, make_data = case(name)
-    B = 64
-    data = make_data(B)
-    spec, keys_spec = _solve_twice(cfg, data, B, 0)
-    gen, keys_gen = _solve_twice(cfg, data, B, 1)
-    assert keys_spec == (capi.MODEL_UNI_POINT, capi.PROBLEM_GENERIC)
-    assert keys_gen == (capi.MODEL_GENERIC, capi.PROBLEM_GENERIC)
-    assert (spec[0]["status"] == capi.STATUS_CONVERGED).sum() >= B // 4, spec[0]["status"]
-    for step, (a, b) in enumerate(zip(spec, gen)):
-        for f in FIELDS:
-            assert np.array_equal(_bits(a[f]), _bits(b[f])), f"step {step}: {f} differs between the specialised and the generic kernels"
 
 
 def _cuda_solve(cfg, data):

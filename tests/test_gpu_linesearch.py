@@ -4,31 +4,22 @@ Every comparison starts from one shared state: the oracle's own iterate j of eac
 device workspace after the device's own INIT and ASSOCIATE (the association must be the oracle's).  EVAL and KKT run on the
 device and are checked with the tolerances of the phase tests; then the oracle's records, step and scalars are written, so
 that both line searches start from the same inputs, and the iterate, the slacks, the multipliers and DT, ALPHA, RHO, NBT, ITER,
-TINY, STATUS are compared (tests/linesearch_cases.py has the tolerances and the rule for decisions at their threshold).
+TINY, STATUS are compared (tests/parity.py has the tolerances and the rule for decisions at their threshold).
 
 Every phase-kernel variant is reached, and the launch reports its model / problem key: <false, MODEL_UNI_POINT_QF>,
 <false, MODEL_UNI_POINT>, <false, MODEL_GENERIC> and <true, MODEL_GENERIC> (line obstacles, moving obstacles, midpoint
 differences), with the unbordered and the bordered KKT (free dt, fixed final-state components).  The horizons cover idle lanes
 of the warp reductions, the cross-warp merges (N > 32) and threads that own two stages (N > 128).  The fused solve kernel is
 not stepped phase by phase: the fused == phased and specialised == generic bit-identity tests (test_gpu_parity,
-test_gpu_model_variants, test_gpu_problem_variants) tie it to these phase kernels."""
-import numpy as np
+test_gpu_model_phases, test_gpu_kernel_keys) tie it to these phase kernels."""
 import pytest
 
 import linesearch_cases as lc
-import test_fixed_final_state as tff
-from mpc_local_planner_b200 import capi, configs
+from fixed_cases import case as fixed_case
+from mpc_local_planner_b200 import configs
+from parity import GEN, UNI, UNI_QF, compare_at
 
 pytestmark = pytest.mark.gpu
-
-UNI_QF = (capi.MODEL_UNI_POINT, capi.PROBLEM_FIXED_DT_QF)
-UNI = (capi.MODEL_UNI_POINT, capi.PROBLEM_GENERIC)
-GEN = (capi.MODEL_GENERIC, capi.PROBLEM_GENERIC)
-
-
-def _fixed(name):
-    make_cfg, make_data = tff.FIXED_CASES[name]
-    return make_cfg(), make_data
 
 
 # name -> (configuration, data(B), force the generic kernels, expected keys)
@@ -37,10 +28,10 @@ VARIANTS = {
     "qf_cfg5": (lambda: lc.case("cfg5")[0], lambda B: configs.generate(5, B), 0, UNI_QF),
     "uni_integral_free_dt": (lambda: lc.case("integral_free_dt")[0], lambda B: configs.generate(2, B), 0, UNI),
     "uni_terminal_ball": (lambda: lc.case("terminal_ball")[0], lambda B: configs.generate(2, B), 0, UNI),
-    "uni_qf_position_fixed": (lambda: _fixed("qf_position_fixed")[0], lambda B: _fixed("qf_position_fixed")[1](B), 0, UNI),
+    "uni_qf_position_fixed": (lambda: fixed_case("qf_position_fixed")[0], lambda B: fixed_case("qf_position_fixed")[1](B), 0, UNI),
     "generic_cfg3": (lambda: lc.case("cfg3")[0], lambda B: configs.generate(3, B), 0, GEN),
     "generic_forced_cfg2": (lambda: lc.case("cfg2")[0], lambda B: configs.generate(2, B), 1, GEN),
-    "generic_trap_position_fixed": (lambda: _fixed("trap_position_fixed")[0], lambda B: _fixed("trap_position_fixed")[1](B), 1, GEN),
+    "generic_trap_position_fixed": (lambda: fixed_case("trap_position_fixed")[0], lambda B: fixed_case("trap_position_fixed")[1](B), 1, GEN),
     "lines": (lambda: lc.case("line_obstacles")[0], lambda B: configs.with_line_obstacles(configs.generate(2, B)), 0, GEN),
     "lines_dynamic_fixed_dt": (lambda: lc.case("dynamic_fixed_dt")[0],
                                lambda B: configs.with_moving_obstacles(configs.generate(2, B)), 0, GEN),
@@ -51,87 +42,6 @@ VARIANTS = {
 }
 
 
-def _oracle_and_compare(cfg, o, dev, dev_scal, what):
-    """the oracle's line search on its shared state, then the device's result against it.  The row values and gradients are
-    the inputs each side computes itself; near convergence the line search magnifies their rounding through 1 / s
-    (linesearch_cases.row_sensitivity)."""
-    pre = {nm: o.arr(nm).copy() for nm in ("S", "LAM", "SCAL")}
-    d = o.linesearch()
-    sens = lc.row_sensitivity(pre, o.arr("G"), o.arr("DS"), d)
-    return lc.assert_same_outcome(cfg, d, {nm: o.arr(nm) for nm, _ in lc.STATE_FIELDS}, o.arr("SCAL"), dev, dev_scal, what,
-                                  sens=sens)
-
-
-def _compare_at(orc, cfg, data, B, j, force_generic=0, keys=None):
-    """one line search on B instances from the oracle's iterate j; returns (compared, marginal) instance counts"""
-    s = capi.BatchSolver(cfg, B, device=0)
-    s.set_option(capi.OPT_FORCE_GENERIC_MODEL, force_generic)
-    s.upload(data["x0"], data["xf"], data["u_prev"], data["u_prev_dt"], data["obstacles"], data["viapoints"])
-    s.run_phase(capi.PHASE_INIT); s.run_phase(capi.PHASE_ASSOCIATE)
-    if keys is not None:
-        assert (s.kernel_model(), s.kernel_problem()) == keys
-    OBS = s.ws_read(capi.F_OBSIDX)
-    inst, live = [], []
-    for b in range(B):
-        o, converged = lc.oracle_iterate(orc, cfg, data, b, j)
-        np.testing.assert_array_equal(OBS[b], o.arr("OBSIDX"))
-        inst.append(o)
-        live.append(not converged)
-    for nm, f in lc.STATE_FIELDS:
-        s.ws_write(f, np.stack([o.arr(nm) for o in inst]))
-    SC = s.ws_read(capi.F_SCAL)
-    s.ws_write(capi.F_SCAL, np.stack([lc.merged_scal(SC[b], inst[b].arr("SCAL")) for b in range(B)]))
-    # EVAL and KKT, checked (records and scalars with the tolerances of test_gpu_parity.test_phase_parity)
-    s.run_phase(capi.PHASE_EVAL)
-    KKT, SC = s.ws_read(capi.F_KKT), s.ws_read(capi.F_SCAL)
-    s.run_phase(capi.PHASE_KKT)
-    STEP, SC2 = s.ws_read(capi.F_STEP), s.ws_read(capi.F_SCAL)
-    rows = lc.step_rows(cfg)
-    for b, o in enumerate(inst):
-        o.eval()
-        if not live[b]:
-            continue
-        scale = np.abs(o.arr("KKT")).max()
-        np.testing.assert_allclose(KKT[b], o.arr("KKT"), rtol=0, atol=1e-11 * scale)
-        idx = list(lc.EVAL_SCAL)
-        np.testing.assert_allclose(SC[b][idx], o.arr("SCAL")[idx], rtol=1e-10, atol=1e-12)
-        if SC2[b][capi.SC_DEFER] != 0.0:
-            o.arr("SCAL")[capi.SC_DEFER] = 1.0   # both take the null step
-            continue
-        if o.kkt_solve(SC2[b][capi.SC_DELTA]) != 0:
-            # an inertia decision at the margin: the line search gets the oracle's own step anyway
-            assert any(o.kkt_solve(dl) == 0 for dl in (1e-4, 1e-2, 1.0, 100.0))
-            continue
-        # (the Newton step of late iterates is ill-conditioned: 6e-8 of its size measured; the emulator tests' tolerance)
-        sscale = max(np.abs(o.arr("STEP")).max(), 1.0)
-        np.testing.assert_allclose(STEP[b][:rows], o.arr("STEP")[:rows], rtol=0, atol=1e-7 * sscale)
-        assert abs(SC2[b][capi.SC_DDT] - o.arr("SCAL")[capi.SC_DDT]) <= 1e-9 * max(1.0, abs(o.arr("SCAL")[capi.SC_DDT]))
-    # identical line-search inputs: the oracle's records, step (the device's heading multiplier row with midpoint
-    # differences) and scalars
-    s.ws_write(capi.F_KKT, np.stack([o.arr("KKT") for o in inst]))
-    STEP = STEP.copy()
-    for b, o in enumerate(inst):
-        STEP[b][:rows] = o.arr("STEP")[:rows]
-    s.ws_write(capi.F_STEP, STEP)
-    SC = s.ws_read(capi.F_SCAL)
-    for b, o in enumerate(inst):
-        if not live[b]:
-            o.arr("SCAL")[capi.SC_STATUS] = SC[b][capi.SC_STATUS]   # converged on both sides: nothing may change
-    s.ws_write(capi.F_SCAL, np.stack([lc.merged_scal(SC[b], inst[b].arr("SCAL")) for b in range(B)]))
-    s.run_phase(capi.PHASE_LINESEARCH)
-    dev = {nm: s.ws_read(f) for nm, f in lc.STATE_FIELDS}
-    DSC = s.ws_read(capi.F_SCAL)
-    if keys is not None:
-        assert (s.kernel_model(), s.kernel_problem()) == keys
-    s.close()
-    compared = marginal = 0
-    for b, o in enumerate(inst):
-        m = _oracle_and_compare(cfg, o, {nm: dev[nm][b] for nm, _ in lc.STATE_FIELDS}, DSC[b], f"instance {b}, iterate {j}")
-        compared += live[b]
-        marginal += m
-    return compared, marginal
-
-
 @pytest.mark.parametrize("variant", list(VARIANTS))
 def test_linesearch_matches_oracle(cuda_lib, orc, variant):
     make_cfg, make_data, force_generic, keys = VARIANTS[variant]
@@ -140,7 +50,7 @@ def test_linesearch_matches_oracle(cuda_lib, orc, variant):
     data = make_data(B)
     compared = marginal = 0
     for j in lc.ITERATES:
-        c, m = _compare_at(orc, cfg, data, B, j, force_generic, keys)
+        c, m = compare_at(orc, cfg, data, B, j, force_generic, keys)
         compared += c; marginal += m
     assert compared >= 12 and marginal <= 2, (compared, marginal)
 
@@ -156,53 +66,20 @@ def test_linesearch_horizons(cuda_lib, orc, cid, n):
     data = configs.generate(cid, B, n=n)
     compared = marginal = 0
     for j in (0, 3, 10):
-        c, m = _compare_at(orc, cfg, data, B, j, 0, UNI_QF if cid == 5 else GEN)
+        c, m = compare_at(orc, cfg, data, B, j, 0, UNI_QF if cid == 5 else GEN)
         compared += c; marginal += m
     assert compared >= 3 and marginal <= 1, (compared, marginal)
 
 
 @pytest.mark.parametrize("edge", [e for e in lc.EDGES if e not in ("kappa_sigma", "flat_merit")])
 def test_linesearch_edge_states(cuda_lib, orc, edge):
-    """the edge states of tests/test_linesearch.py on the fixed-dt quadratic-form and the generic kernels"""
+    """the edge states of tests/test_linesearch.py on the fixed-dt quadratic-form and the generic kernels, from iterate 3: no
+    deferred step, the inertia right at the device's regularisation"""
     _, post = lc.EDGES[edge]
     for variant in ("qf_cfg2", "generic_cfg3"):
         make_cfg, make_data, force_generic, keys = VARIANTS[variant]
         cfg = make_cfg()
         B = 2
         data = make_data(B)
-        c, m = _compare_edge(orc, cfg, data, B, post, force_generic, keys)
+        c, m = compare_at(orc, cfg, data, B, 3, force_generic, keys, post)
         assert c >= 1 and m == 0
-
-
-def _compare_edge(orc, cfg, data, B, post, force_generic, keys):
-    """as _compare_at at iterate 3, with the edge change applied to the oracle's state after its Newton step"""
-    s = capi.BatchSolver(cfg, B, device=0)
-    s.set_option(capi.OPT_FORCE_GENERIC_MODEL, force_generic)
-    s.upload(data["x0"], data["xf"], data["u_prev"], data["u_prev_dt"], data["obstacles"], data["viapoints"])
-    s.run_phase(capi.PHASE_INIT); s.run_phase(capi.PHASE_ASSOCIATE)
-    inst = [lc.oracle_iterate(orc, cfg, data, b, 3)[0] for b in range(B)]
-    for nm, f in lc.STATE_FIELDS:
-        s.ws_write(f, np.stack([o.arr(nm) for o in inst]))
-    SC = s.ws_read(capi.F_SCAL)
-    s.ws_write(capi.F_SCAL, np.stack([lc.merged_scal(SC[b], inst[b].arr("SCAL")) for b in range(B)]))
-    s.run_phase(capi.PHASE_EVAL); s.run_phase(capi.PHASE_KKT)
-    SC2, STEP = s.ws_read(capi.F_SCAL), s.ws_read(capi.F_STEP).copy()
-    for b, o in enumerate(inst):
-        o.eval()
-        assert SC2[b][capi.SC_DEFER] == 0.0 and o.kkt_solve(SC2[b][capi.SC_DELTA]) == 0
-        post(o)
-        STEP[b][:lc.step_rows(cfg)] = o.arr("STEP")[:lc.step_rows(cfg)]
-    s.ws_write(capi.F_KKT, np.stack([o.arr("KKT") for o in inst]))
-    s.ws_write(capi.F_STEP, STEP)
-    s.ws_write(capi.F_SCAL, np.stack([lc.merged_scal(SC2[b], inst[b].arr("SCAL")) for b in range(B)]))
-    before = [o.arr("SCAL").copy() for o in inst]
-    s.run_phase(capi.PHASE_LINESEARCH)
-    assert (s.kernel_model(), s.kernel_problem()) == keys
-    dev = {nm: s.ws_read(f) for nm, f in lc.STATE_FIELDS}
-    DSC = s.ws_read(capi.F_SCAL)
-    s.close()
-    compared = marginal = 0
-    for b, o in enumerate(inst):
-        marginal += _oracle_and_compare(cfg, o, {nm: dev[nm][b] for nm, _ in lc.STATE_FIELDS}, DSC[b], f"instance {b}")
-        compared += 1
-    return compared, marginal

@@ -3,6 +3,8 @@ Tolerance (BASELINE.json north_star): |u* - u*_oracle|_inf < 1e-4 at converged K
 import numpy as np
 import pytest
 
+import costmap_cases as cm
+import parity as par
 from mpc_local_planner_b200 import capi, configs
 
 pytestmark = pytest.mark.gpu
@@ -17,54 +19,13 @@ def _solver(cfg, B):
     return capi.BatchSolver(cfg, B, device=0)
 
 
-def _load_inputs(solver, data):
-    solver.upload(data["x0"], data["xf"], data["u_prev"], data["u_prev_dt"], data["obstacles"], data["viapoints"])
-
-
-def _oracle_state(orc, cfg, data, b, n_iters):
-    """oracle instance advanced by n_iters full interior-point iterations (cold start)"""
-    o = orc.instance_from_batch(cfg, data, b)
-    o.init_cold(); o.associate()
-    o.L.orc_project_init(orc.C.byref(o.p), o.ws); o.L.orc_init_controls(orc.C.byref(o.p), o.ws)
-    o.init_duals()
-    return o
-
-
 @pytest.mark.parametrize("cid,B", [(1, 1), (2, 8), (3, 6), (4, 6)])
 def test_phase_parity(cuda_lib, orc, cid, B):
-    """INIT/ASSOCIATE/EVAL/KKT outputs of the kernels match the oracle field by field on the same iterate."""
+    """INIT/ASSOCIATE/EVAL/KKT outputs of the kernels match the oracle field by field at the first iterate; the step at the
+    regularisation the kernel settled on."""
     cfg = configs.config_for(cid, tol=1e-8)
     data = _data(cid, B)
-    s = _solver(cfg, B)
-    _load_inputs(s, data)
-    s.run_phase(capi.PHASE_INIT); s.run_phase(capi.PHASE_ASSOCIATE)
-    X, U, S, LAM, OBS = (s.ws_read(f) for f in (capi.F_X, capi.F_U, capi.F_S, capi.F_LAM, capi.F_OBSIDX))
-    s.run_phase(capi.PHASE_EVAL)
-    KKT, SC = s.ws_read(capi.F_KKT), s.ws_read(capi.F_SCAL)
-    s.run_phase(capi.PHASE_KKT)
-    STEP, SC2 = s.ws_read(capi.F_STEP), s.ws_read(capi.F_SCAL)
-    for b in range(B):
-        o = _oracle_state(orc, cfg, data, b, 0)
-        np.testing.assert_allclose(X[b], o.arr("X"), rtol=0, atol=1e-12)
-        np.testing.assert_allclose(U[b], o.arr("U"), rtol=0, atol=1e-12)
-        np.testing.assert_array_equal(OBS[b], o.arr("OBSIDX"))
-        np.testing.assert_allclose(S[b], o.arr("S"), rtol=1e-11, atol=1e-13)
-        np.testing.assert_allclose(LAM[b], o.arr("LAM"), rtol=1e-10, atol=1e-13)
-        o.eval()
-        scale = np.abs(o.arr("KKT")).max()
-        np.testing.assert_allclose(KKT[b], o.arr("KKT"), rtol=0, atol=1e-11 * scale)
-        idx = [capi.SC_MU, capi.SC_HTT, capi.SC_GT, capi.SC_ERR0, capi.SC_ERRMU, capi.SC_OBJ, capi.SC_INF, capi.SC_BLOG]
-        np.testing.assert_allclose(SC[b][idx], o.arr("SCAL")[idx], rtol=1e-10, atol=1e-12)
-        if SC2[b][capi.SC_DEFER] != 0.0:
-            assert o.kkt_solve(0.0) == 1  # factorisation budget spent at this iterate: wrong inertia at delta = 0 for both
-        elif SC2[b][capi.SC_DELTA] == 0.0:
-            assert o.kkt_solve(0.0) == 0
-            sscale = np.abs(o.arr("STEP")).max()
-            np.testing.assert_allclose(STEP[b], o.arr("STEP"), rtol=0, atol=1e-9 * sscale)
-            assert abs(SC2[b][capi.SC_DDT] - o.arr("SCAL")[capi.SC_DDT]) <= 1e-9 * max(1.0, abs(o.arr("SCAL")[capi.SC_DDT]))
-        else:
-            assert o.kkt_solve(0.0) == 1  # both see the wrong inertia at delta = 0
-    s.close()
+    par.check_first_iterate(orc, cfg, data, B)
 
 
 @pytest.mark.parametrize("cid,B", [(1, 1), (2, 64), (3, 24), (4, 32), (5, 16)])
@@ -331,14 +292,13 @@ def test_line_obstacles(cuda_lib, orc, cid, B):
     """LineObstacle rows through the C ABI: records of the first evaluation and whole solves against the oracle."""
     cfg = configs.config_for(cid, tol=1e-8)
     data = configs.with_line_obstacles(configs.generate(cid, B))
-    s = _solver(cfg, B)
-    _load_inputs(s, data)
+    s = par.phase_solver(cfg, data, B)
     s.run_phase(capi.PHASE_INIT); s.run_phase(capi.PHASE_ASSOCIATE)
     X, OBS = s.ws_read(capi.F_X), s.ws_read(capi.F_OBSIDX)
     s.run_phase(capi.PHASE_EVAL)
     KKT = s.ws_read(capi.F_KKT)
     for b in range(0, B, 4):
-        o = _oracle_state(orc, cfg, data, b, 0)
+        o = par.oracle_init(orc, cfg, data, b)
         np.testing.assert_allclose(X[b], o.arr("X"), rtol=0, atol=1e-12)
         np.testing.assert_array_equal(OBS[b], o.arr("OBSIDX"))
         o.eval()
@@ -425,21 +385,13 @@ def test_dynamic_obstacles(cuda_lib, orc, free_dt):
 @pytest.mark.parametrize("cid,B", [(2, 96), (3, 40)])
 def test_fused_and_phased_solves_are_identical(cuda_lib, cid, B):
     """One persistent kernel per solve (default) or one kernel launch per phase is an execution choice only: the same
-    device functions run in the same order, so statuses, iteration counts and controls are identical bit for bit."""
+    device functions run in the same order, so every output of a cold and then a warm solve is identical bit for bit."""
     cfg = configs.config_for(cid, tol=1e-8)
     data = _data(cid, B)
-    outs = []
-    for mode in (capi.SOLVE_FUSED, capi.SOLVE_PHASED):
-        s = _solver(cfg, B)
-        s.set_option(capi.OPT_SOLVE_MODE, mode)
-        outs.append(s.step(data["x0"], data["xf"], data["u_prev"], data["u_prev_dt"], data["obstacles"], data["viapoints"]))
-        s.close()
-    a, b = outs
-    np.testing.assert_array_equal(a["status"], b["status"])
-    np.testing.assert_array_equal(a["iters"], b["iters"])
-    np.testing.assert_array_equal(a["u_seq"], b["u_seq"])
-    np.testing.assert_array_equal(a["x_seq"], b["x_seq"])
-    np.testing.assert_array_equal(a["dt"], b["dt"])
+    fused, keys_f = par.solve_twice(cfg, data, B, capi.SOLVE_FUSED)
+    phased, keys_p = par.solve_twice(cfg, data, B, capi.SOLVE_PHASED)
+    assert keys_f == keys_p
+    par.assert_same_solves(fused, phased, "the fused and the phased solve")
 
 
 @pytest.mark.gpu
@@ -534,10 +486,9 @@ def test_midpoint_differences(cuda_lib, orc, base):
 @pytest.mark.parametrize("W,H", [(203, 97), (64, 33), (5, 2), (130, 300)])
 def test_costmap_obstacles_odd_sizes(cuda_lib, orc, W, H):
     """map widths that are not a multiple of four (byte path of the marking kernel), heights around the 32-row mask words"""
-    from test_oracle_functions import _random_costmap
     rng = np.random.default_rng(W + 7 * H)
     B, res = 6, 0.1
-    cost = np.stack([_random_costmap(rng, W, H, 0.03) for _ in range(B)])
+    cost = np.stack([cm.random_costmap(rng, W, H, 0.03) for _ in range(B)])
     origin = rng.uniform(-3, 3, (B, 2))
     pose = np.concatenate([origin + 0.5 * res * np.array([W, H]) + rng.uniform(-1, 1, (B, 2)), rng.uniform(-np.pi, np.pi, (B, 1))], axis=1)
     s = _solver(configs.cfg2(), 1)
@@ -553,10 +504,9 @@ def test_costmap_obstacles_odd_sizes(cuda_lib, orc, W, H):
 def test_costmap_obstacles_match_oracle_and_feed_the_solver(cuda_lib, orc):
     """mpcb200_costmap_obstacles (updateObstacleContainerWithCostmap for a batch of robots) against the oracle's loops: same
     cells, same order, same cut; the lists then go straight into step() as its obstacles."""
-    from test_oracle_functions import _random_costmap
     rng = np.random.default_rng(5)
     B, W, H, res = 24, 200, 160, 0.05
-    cost = np.stack([_random_costmap(rng, W, H, 0.002) for _ in range(B)])
+    cost = np.stack([cm.random_costmap(rng, W, H, 0.002) for _ in range(B)])
     for b in range(B):
         cost[b, :, W - 1] = 0; cost[b, H - 1, :] = 0
     cost[0] = 0                      # an empty map

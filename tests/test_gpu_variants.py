@@ -7,6 +7,7 @@ Each case: the CUDA path through the C ABI against the CPU oracle on the same se
 import numpy as np
 import pytest
 
+import costmap_cases as cm
 from mpc_local_planner_b200 import capi, configs
 
 pytestmark = pytest.mark.gpu
@@ -183,10 +184,9 @@ def test_check_feasible_matches_the_oracle(cuda_lib, orc, footprint):
     """mpcb200_check_feasible (Controller::isPoseTrajectoryFeasible, controller.cpp:859-917) for a batch of robots: accept /
     reject byte for byte as the oracle's plain-C loop, on random maps, trajectories that turn and leave the map, both look-ahead
     settings -- and on the trajectories of a solve that are still on the device."""
-    from tests.test_oracle_functions import _feasibility_cases
     rng = np.random.default_rng(5)
     fp = np.array(configs.CARLIKE_POLYGON) if footprint == "polygon" else np.array([[0.1, 0.0], [-0.1, 0.0]])
-    cases = _feasibility_cases(rng, 96)
+    cases = cm.feasibility_cases(rng, 96)
     cost = np.stack([c[0] for c in cases]); origin = np.stack([c[1] for c in cases]); xs = np.stack([c[2] for c in cases])
     cfg = configs.cfg2(tol=1e-6)
     s = capi.BatchSolver(cfg, 96, device=0)
@@ -238,31 +238,13 @@ def test_multi_device_handle_equals_single_device(cuda_lib):
     m.close()
 
 
-def _costmap_scene(B, density, seed, ahead=3.0):
-    """robots on random costmaps, goals 3 m ahead, the cells around start and goal cleared"""
-    from test_oracle_functions import _random_costmap
-    rng = np.random.default_rng(seed)
-    W, H, res = 200, 160, 0.05
-    cost = np.stack([_random_costmap(rng, W, H, density) for _ in range(B)])
-    cost[:, :, W - 1] = 0; cost[:, H - 1, :] = 0
-    origin = rng.uniform(-3, 3, (B, 2))
-    pose = np.concatenate([origin + rng.uniform(2.5, 4.5, (B, 2)), rng.uniform(-np.pi, np.pi, (B, 1))], axis=1)
-    goal = pose.copy(); goal[:, 0] += ahead * np.cos(pose[:, 2]); goal[:, 1] += ahead * np.sin(pose[:, 2])
-    yy, xx = np.mgrid[0:H, 0:W]
-    for b in range(B):
-        cx, cy = origin[b, 0] + (xx + 0.5) * res, origin[b, 1] + (yy + 0.5) * res
-        for p in (pose[b], goal[b]):
-            cost[b][(cx - p[0]) ** 2 + (cy - p[1]) ** 2 < 0.7 ** 2] = 0
-    return cost, origin, res, pose, goal
-
-
 def test_long_obstacle_lists_stay_in_global_memory(cuda_lib, orc):
     """SURVEY 8 f-1, second half: the raw costmap list of a robot (hundreds of point obstacles, far beyond the 64 resident
     slots) goes into step() as it is.  The association runs over the list in global memory (StageInequalitySE2::update,
     stage_inequality_se2.cpp:73-147) and only what it selects becomes resident: same rows per stage as the oracle's loop over the
     full list, same cold start (the bumps look at the full list as well), same solves."""
     B, M = 16, 512
-    cost, origin, res, pose, goal = _costmap_scene(B, 0.006, 11)
+    cost, origin, res, pose, goal = cm.costmap_scene(B, 0.006, 11)
     cfg = configs.cfg2(tol=1e-6)
     s = capi.BatchSolver(cfg, B, device=0)
     (count, typ, par), found = s.costmap_obstacles(cost, origin, res, pose, 0.3, M)
@@ -324,7 +306,7 @@ def test_resident_list_overflow_is_counted(cuda_lib):
     """a map so dense that the union of the selected obstacles exceeds the resident list: rows are dropped, counted, and the
     solve still ends in a defined status"""
     B, M = 4, 2048
-    cost, origin, res, pose, goal = _costmap_scene(B, 0.12, 12, ahead=4.5)
+    cost, origin, res, pose, goal = cm.costmap_scene(B, 0.12, 12, ahead=4.5)
     cfg = configs.cfg2(tol=1e-6)
     cfg.k_max_obstacles_per_stage = 8
     s = capi.BatchSolver(cfg, B, device=0)

@@ -9,8 +9,9 @@
 import numpy as np
 import pytest
 
+import dense_kkt as dk
 import linesearch_cases as lc
-import test_oracle_functions as tof
+import parity as par
 from mpc_local_planner_b200 import capi
 
 # ---- the oracle's line search against independent checks -------------------------------------------------------------
@@ -21,7 +22,7 @@ DJ_CASES = ["cfg2", "integral_fixed_dt", "integral_free_dt", "trapezoid_fixed_dt
 
 def _oracle_step(orc, cfg, data, b, j):
     """the oracle's iterate j, evaluated and factorised (the solve's first inertia attempt, else the next regularisations)"""
-    o, _ = lc.oracle_iterate(orc, cfg, data, b, j)
+    o, _ = par.oracle_iterate(orc, cfg, data, b, j)
     o.eval()
     dl = o.arr("SCAL")[capi.SC_DELTA_LAST]
     for delta in ([dl / 3.0] if dl > 0 else []) + [0.0, 1e-4, 1e-2, 1.0, 100.0]:
@@ -57,8 +58,8 @@ def test_curvature_matches_the_dense_hessian(orc, cid):
     """curv = dz'(H + delta I)dz + sum sigma ds^2, with H the condensed Hessian of the dense KKT system (finite differences of
     the analytic gradient, the same assembly the Newton-step test uses): the block, the control-rate cross blocks and the dt
     border of the stage records."""
-    inst, cfg = tof._random_iterate(orc, cid, 1, 0, 0.05)
-    Hc, _, _, _, free = tof._dense_kkt(inst, cfg)
+    inst, cfg = dk.random_iterate(orc, cid, 1, 0, 0.05)
+    Hc, _, _, _, free = dk.dense_kkt(inst, cfg)
     N = inst.N
     for delta in (0.0, 1e-2, 1.0, 100.0):
         if inst.kkt_solve(delta) == 0:
@@ -143,64 +144,6 @@ def test_step_length_rules(orc, name):
 
 # ---- the device code (CPU warp emulator) against the oracle -----------------------------------------------------------
 
-def emu_from_oracle(emu, cfg, data, b, o):
-    """an emulator instance with the device's own initialisation and association, then the oracle's iterate"""
-    e = emu.instance_from_batch(cfg, data, b)
-    e.init(); e.associate()
-    np.testing.assert_array_equal(e.field(capi.F_OBSIDX), o.arr("OBSIDX"))
-    for nm, f in lc.STATE_FIELDS:
-        e.set_field(f, o.arr(nm))
-    e.set_field(capi.F_SCAL, lc.merged_scal(e.field(capi.F_SCAL), o.arr("SCAL")))
-    return e
-
-
-def eval_and_kkt(o, e, cfg, step_tol=1e-7):
-    """EVAL and KKT on both sides, compared with the tolerances of the phase tests; False when the device defers the step"""
-    o.eval(); e.eval()
-    scale = np.abs(o.arr("KKT")).max()
-    np.testing.assert_allclose(e.field(capi.F_KKT), o.arr("KKT"), atol=1e-9 * scale)
-    idx = list(lc.EVAL_SCAL)
-    np.testing.assert_allclose(e.field(capi.F_SCAL)[idx], o.arr("SCAL")[idx], rtol=1e-8, atol=1e-10)
-    assert e.kkt() == 0
-    if e.field(capi.F_SCAL)[capi.SC_DEFER] != 0.0:
-        return False
-    if o.kkt_solve(e.field(capi.F_SCAL)[capi.SC_DELTA]) != 0:
-        # an inertia decision at the margin (seen on rounding-sized steps): the line search gets the oracle's step anyway
-        assert step_tol > 1e-7 and any(o.kkt_solve(dl) == 0 for dl in (1e-4, 1e-2, 1.0, 100.0))
-        return True
-    rows = lc.step_rows(cfg)
-    sscale = max(np.abs(o.arr("STEP")).max(), 1.0)
-    np.testing.assert_allclose(e.field(capi.F_STEP)[:rows], o.arr("STEP")[:rows], atol=step_tol * sscale)
-    ddt = o.arr("SCAL")[capi.SC_DDT]
-    assert abs(e.field(capi.F_SCAL)[capi.SC_DDT] - ddt) <= 1e-2 * step_tol * max(1.0, abs(ddt))
-    return True
-
-
-def share_inputs(o, e, cfg):
-    """the oracle's records, step and scalars into the emulator: both line searches start from bit-identical inputs"""
-    e.set_field(capi.F_KKT, o.arr("KKT"))
-    rows = lc.step_rows(cfg)
-    STEP = e.field(capi.F_STEP).copy()
-    STEP[:rows] = o.arr("STEP")[:rows]
-    e.set_field(capi.F_STEP, STEP)
-    e.set_field(capi.F_SCAL, lc.merged_scal(e.field(capi.F_SCAL), o.arr("SCAL")))
-
-
-def run_both(o, e, cfg, what, post=None, rho_tol=1e-10):
-    """share the inputs, run one line search on each side, compare; returns (diagnostics, marginal, SCAL before)"""
-    if post is not None:
-        post(o)
-    share_inputs(o, e, cfg)
-    pre = {nm: o.arr(nm).copy() for nm in ("S", "LAM", "SCAL")}
-    d = o.linesearch()
-    e.linesearch()
-    sens = lc.row_sensitivity(pre, o.arr("G"), o.arr("DS"), d)
-    marginal = lc.assert_same_outcome(cfg, d, {nm: o.arr(nm) for nm, _ in lc.STATE_FIELDS}, o.arr("SCAL"),
-                                      {nm: e.field(f) for nm, f in lc.STATE_FIELDS}, e.field(capi.F_SCAL), what,
-                                      rho_tol=rho_tol, sens=sens)
-    return d, marginal, pre["SCAL"]
-
-
 @pytest.mark.parametrize("name", list(lc.CASES))
 def test_device_linesearch_matches_oracle(orc, emu, name):
     """Iterates 0, 1, 3, 10, 25 and the last before convergence of one instance; at most one of the six may put a discrete
@@ -208,13 +151,13 @@ def test_device_linesearch_matches_oracle(orc, emu, name):
     cfg, data, b = lc.case(name)
     n_marginal = n_compared = 0
     for j in lc.ITERATES:
-        o, converged = lc.oracle_iterate(orc, cfg, data, b, j)
+        o, converged = par.oracle_iterate(orc, cfg, data, b, j)
         if converged:   # before iterate j
             continue
-        e = emu_from_oracle(emu, cfg, data, b, o)
-        if not eval_and_kkt(o, e, cfg):
+        e = par.emu_from_oracle(emu, cfg, data, b, o)
+        if not par.eval_and_kkt(o, e, cfg):
             continue
-        _, marginal, _ = run_both(o, e, cfg, f"{name} iterate {j}")
+        _, marginal, _ = par.run_both(o, e, cfg, f"{name} iterate {j}")
         n_marginal += marginal
         n_compared += 1
     assert n_compared >= 3 and n_marginal <= 1, (n_compared, n_marginal)
@@ -223,6 +166,10 @@ def test_device_linesearch_matches_oracle(orc, emu, name):
 # (not midpoint differences: the heading multiplier row of their step is the device's own, and a changed step would leave it
 # inconsistent with the oracle's)
 EDGE_CASES = ["cfg1", "cfg2", "cfg3", "integral_free_dt"]
+# multipliers 1e12 times too large (kappa_sigma) make the Newton step ill-conditioned, and so is the rounding-sized step of
+# iterate 60 (flat_merit); the line search gets the oracle's step anyway
+ILL_CONDITIONED_STEP = (1e-4, 1.0)
+ILL_CONDITIONED_DDT = 1e-6
 
 
 @pytest.mark.parametrize("edge", list(lc.EDGES))
@@ -236,14 +183,16 @@ def test_device_linesearch_edge_states(orc, emu, edge):
         j = 3
         if edge == "flat_merit":
             cfg.tol, j = 1e-15, 60
-        o, _ = lc.oracle_iterate(orc, cfg, data, b, j)
+        o, _ = par.oracle_iterate(orc, cfg, data, b, j)
         if pre is not None:
             pre(o)
-        e = emu_from_oracle(emu, cfg, data, b, o)
-        # (multipliers 1e12 times too large make the Newton step ill-conditioned; the line search gets the oracle's anyway)
-        assert eval_and_kkt(o, e, cfg, step_tol=1e-4 if edge in ("kappa_sigma", "flat_merit") else 1e-7)
+        e = par.emu_from_oracle(emu, cfg, data, b, o)
+        if edge in ("kappa_sigma", "flat_merit"):
+            assert par.eval_and_kkt(o, e, cfg, ILL_CONDITIONED_STEP, ILL_CONDITIONED_DDT)
+        else:
+            assert par.eval_and_kkt(o, e, cfg)
         # (rho sums sigma ds^2: multipliers 1e12 times too large magnify the rounding of ds by as much)
-        d, marginal, before = run_both(o, e, cfg, f"{name}, {edge}", post, rho_tol=1e-5 if edge == "kappa_sigma" else 1e-10)
+        d, marginal, before = par.run_both(o, e, cfg, f"{name}, {edge}", post, rho_tol=1e-5 if edge == "kappa_sigma" else 1e-10)
         # the flat-merit test compares a rounding-sized merit change with its bound: that decision is marginal by design
         assert not marginal or edge == "flat_merit"
         lc.check_edge(edge, d, before, o.arr("SCAL"))
@@ -290,10 +239,10 @@ def test_threshold_bin_with_exactly_m_over_8_clipped_rows(orc, emu):
         f = _threshold_scale(orc, cfg, data, b)
         if f is None:
             continue
-        o, _ = lc.oracle_iterate(orc, cfg, data, b, 3)
-        e = emu_from_oracle(emu, cfg, data, b, o)
-        assert eval_and_kkt(o, e, cfg)
-        d, marginal, _ = run_both(o, e, cfg, f"{name}, step x {f:.6g}", lc.scale_step(f))
+        o, _ = par.oracle_iterate(orc, cfg, data, b, 3)
+        e = par.emu_from_oracle(emu, cfg, data, b, o)
+        assert par.eval_and_kkt(o, e, cfg)
+        d, marginal, _ = par.run_both(o, e, cfg, f"{name}, step x {f:.6g}", lc.scale_step(f))
         assert not marginal
         # (the search used the oracle's own regularisation; where the device's differs, the step and the counts do too)
         jt = d["jt"]

@@ -7,10 +7,9 @@ kernels."""
 import numpy as np
 import pytest
 
-import linesearch_cases as lc
+import dense_kkt as dk
 import model_cases as mc
-import test_linesearch as tls
-import test_oracle_functions as tof
+import parity as par
 from mpc_local_planner_b200 import capi
 
 B0 = mc.INSTANCE
@@ -22,11 +21,10 @@ def _n_vp(data, b):
 
 
 def assert_association(o, e, cfg, data, b, what):
-    np.testing.assert_array_equal(e.field(capi.F_OBSIDX), o.arr("OBSIDX"), err_msg=what)
+    """INIT / ASSOCIATE (states, controls, association, slacks, multipliers), the via-point stages, dt and mu"""
+    par.assert_init(*par.emu_init_fields(e), o, par.EMU, what)
     if mc.has_viapoints(cfg):
         np.testing.assert_array_equal(e.vp_stage(_n_vp(data, b)), o.vp_stage(), err_msg=what)
-    np.testing.assert_allclose(e.field(capi.F_S), o.arr("S"), rtol=1e-9, err_msg=what)
-    np.testing.assert_allclose(e.field(capi.F_LAM), o.arr("LAM"), rtol=1e-9, err_msg=what)
     np.testing.assert_allclose(e.field(capi.F_SCAL)[list(INIT_SCAL)], o.arr("SCAL")[list(INIT_SCAL)], rtol=1e-12, err_msg=what)
 
 
@@ -34,79 +32,41 @@ def assert_association(o, e, cfg, data, b, what):
 @pytest.mark.parametrize("name", list(mc.CASES))
 def test_newton_step_matches_dense_kkt(orc, name):
     """Analytic Lagrangian gradient vs finite differences and the Riccati step vs a dense numpy solve of the KKT system
-    assembled by finite differences, at multipliers of size 1 and 0.05 (test_oracle_functions).  N = 20 keeps the dense system
+    assembled by finite differences, at multipliers of size 1 and 0.05 (tests/dense_kkt.py).  N = 20 keeps the dense system
     small."""
     cfg, data, _ = mc.case(name, n=20, B=2)
     compared = 0
     for nu_scale in (1.0, 0.05):
-        compared += tof._check_gradient_and_newton_step(orc, None, nu_scale, cfg=cfg, data=data, b=B0)
+        compared += dk.check_gradient_and_newton_step(orc, None, nu_scale, cfg=cfg, data=data, b=B0)
     if compared == 0:   # every regularisation gave the wrong inertia on this iterate: another instance and seed
-        compared += tof._check_gradient_and_newton_step(orc, None, 0.05, cfg=cfg, data=data, b=0, seed=1)
+        compared += dk.check_gradient_and_newton_step(orc, None, 0.05, cfg=cfg, data=data, b=0, seed=1)
     assert compared >= 1
 
 
 # ---- the device code against the oracle, phase by phase ----
-def _share_state(o, e):
-    for nm, f in lc.STATE_FIELDS:
-        e.set_field(f, o.arr(nm))
-    e.set_field(capi.F_SCAL, lc.merged_scal(e.field(capi.F_SCAL), o.arr("SCAL")))
-
-
-def _iterate(o, e, cfg, what):
-    """one interior-point iteration on both sides from a shared state: records, scalars and association after EVAL, the step
-    after KKT, then one line search each from the oracle's records, step and scalars; returns (stepped, marginal)"""
-    o.eval(); e.eval()
-    np.testing.assert_array_equal(e.field(capi.F_OBSIDX), o.arr("OBSIDX"))
-    scale = np.abs(o.arr("KKT")).max()
-    np.testing.assert_allclose(e.field(capi.F_KKT), o.arr("KKT"), atol=1e-9 * scale, err_msg=what)
-    idx = list(lc.EVAL_SCAL)
-    np.testing.assert_allclose(e.field(capi.F_SCAL)[idx], o.arr("SCAL")[idx], rtol=1e-8, atol=1e-10, err_msg=what)
-    assert e.kkt() == 0
-    for i in (capi.SC_DELTA_LAST, capi.SC_NREG):   # the emulator's regularisation bookkeeping is the one both continue with
-        o.arr("SCAL")[i] = e.field(capi.F_SCAL)[i]
-    if e.field(capi.F_SCAL)[capi.SC_DEFER] != 0.0:
-        nxt = e.field(capi.F_SCAL)[capi.SC_DELTA_LAST] / 3.0
-        assert o.kkt_solve(nxt / 8.0) == 1 or o.kkt_solve(nxt / 100.0) == 1
-        o.arr("SCAL")[capi.SC_DEFER] = 1.0
-        _, marginal, _ = tls.run_both(o, e, cfg, f"{what} (null step)")
-        return False, marginal
-    assert o.kkt_solve(e.field(capi.F_SCAL)[capi.SC_DELTA]) == 0
-    rows = lc.step_rows(cfg)
-    sscale = max(np.abs(o.arr("STEP")).max(), 1.0)
-    np.testing.assert_allclose(e.field(capi.F_STEP)[:rows], o.arr("STEP")[:rows], atol=1e-7 * sscale, err_msg=what)
-    ddt = o.arr("SCAL")[capi.SC_DDT]
-    assert e.field(capi.F_SCAL)[capi.SC_DDT] == pytest.approx(ddt, abs=1e-9 * max(1.0, abs(ddt)))
-    _, marginal, _ = tls.run_both(o, e, cfg, what)
-    return True, marginal
-
-
 @pytest.mark.parametrize("name", list(mc.CASES))
 def test_phases_match_oracle(orc, emu, name):
     """INIT and ASSOCIATE (states, controls, association, via-point stages, slacks, multipliers, mu), then four iterations
     in lockstep; then the oracle's iterate 10 re-associated on both sides (no cold-start repair: the association of every
     outer iteration after the first) and four more iterations from there."""
     cfg, data, _ = mc.case(name)
-    o = lc.oracle_init(orc, cfg, data, B0)
+    o = par.oracle_init(orc, cfg, data, B0)
     e = emu.instance_from_batch(cfg, data, B0)
     e.init(); e.associate()
-    np.testing.assert_allclose(e.field(capi.F_X), o.arr("X"), atol=1e-13)
-    np.testing.assert_allclose(e.field(capi.F_U), o.arr("U"), atol=1e-13)
     assert_association(o, e, cfg, data, B0, "cold")
     steps = marginal = 0
     for it in range(4):
-        s, m = _iterate(o, e, cfg, f"{name}, iteration {it}")
+        s, m = par.emu_iterate(o, e, cfg, f"{name}, iteration {it}")
         steps += s; marginal += m
-        _share_state(o, e)
-    o, converged = lc.oracle_iterate(orc, cfg, data, B0, 10)
-    _share_state(o, e)
+    o, converged = par.oracle_iterate(orc, cfg, data, B0, 10)
+    par.emu_set_state(e, o)
     o.associate(); o.init_duals()
     e.associate(first_outer=False)
     assert_association(o, e, cfg, data, B0, "iterate 10, re-associated")
     if not converged:
         for it in range(4):
-            s, m = _iterate(o, e, cfg, f"{name}, re-associated, iteration {it}")
+            s, m = par.emu_iterate(o, e, cfg, f"{name}, re-associated, iteration {it}")
             steps += s; marginal += m
-            _share_state(o, e)
     assert steps >= 3 and marginal <= 1, (steps, marginal)
 
 
@@ -159,13 +119,13 @@ def _edge_state(orc, name, B):
     if name in mc.STEERING_EDGES:
         base, bound = mc.STEERING_EDGES[name]
         cfg, data, _ = mc.case(base, B=B)
-        o, _ = lc.oracle_iterate(orc, cfg, data, b, mc.EDGE_ITERATE)
+        o, _ = par.oracle_iterate(orc, cfg, data, b, mc.EDGE_ITERATE)
         return cfg, data, o, mc.steer_stage(o, cfg, bound)
     cfg, data = mc.edge_data(name, B)
     _, _, otype, pose = mc.EDGES[name]
-    o, _ = lc.oracle_iterate(orc, cfg, data, b, mc.EDGE_ITERATE)
-    cnt, typ, par = data["obstacles"]
-    return cfg, data, o, mc.place_stage(o, otype, pose, typ[b, :cnt[b]], par[b, :cnt[b]])
+    o, _ = par.oracle_iterate(orc, cfg, data, b, mc.EDGE_ITERATE)
+    cnt, typ, prm = data["obstacles"]
+    return cfg, data, o, mc.place_stage(o, otype, pose, typ[b, :cnt[b]], prm[b, :cnt[b]])
 
 
 @pytest.mark.parametrize("name", list(mc.EDGES) + list(mc.STEERING_EDGES))
@@ -176,8 +136,8 @@ def test_edge_states_match_oracle(orc, emu, name):
     the records' scale as well: the arithmetic of its obstacle rows is exact."""
     for B in (1, 2):
         cfg, data, o, k = _edge_state(orc, name, B)
-        e = tls.emu_from_oracle(emu, cfg, data, B - 1, o)
-        tls.eval_and_kkt(o, e, cfg)
+        e = par.emu_from_oracle(emu, cfg, data, B - 1, o)
+        par.eval_and_kkt(o, e, cfg)
         scale = np.abs(o.arr("KKT")).max()
         np.testing.assert_allclose(e.field(capi.F_KKT)[:, k], o.arr("KKT")[:, k], atol=1e-12 * scale, err_msg=f"stage {k}")
 
@@ -191,14 +151,14 @@ def test_via_point_ties_match_oracle(orc, emu, name, n):
     cfg = make_cfg(n)
     data = make_data(2, n)
     for b in range(2):
-        o, _ = lc.oracle_iterate(orc, cfg, data, b, 3)
+        o, _ = par.oracle_iterate(orc, cfg, data, b, 3)
         stages = mc.via_point_tie(o, data, b)
-        e = tls.emu_from_oracle(emu, cfg, data, b, o)
+        e = par.emu_from_oracle(emu, cfg, data, b, o)
         o.associate(); o.init_duals()
         e.associate(first_outer=False)
         assert_association(o, e, cfg, data, b, f"instance {b}")
         assert o.vp_stage()[0] == stages[0], (o.vp_stage(), stages)
-        tls.eval_and_kkt(o, e, cfg)
+        par.eval_and_kkt(o, e, cfg)
 
 
 @pytest.mark.parametrize("name", ["front_quadratic", "front_min_time", "bicycle_quadratic", "bicycle_min_time"])
@@ -208,13 +168,8 @@ def test_init_controls_of_a_standing_plan(orc, emu, name):
     cfg, data, _ = mc.case(name, B=2)
     for b in range(2):
         xi = mc.standing_plan(cfg, data, b)
-        o = orc.instance_from_batch(cfg, data, b)
-        o.init_cold(xi); o.associate()
-        o.L.orc_project_init(orc.C.byref(o.p), o.ws); o.L.orc_init_controls(orc.C.byref(o.p), o.ws)
-        o.init_duals()
+        o = par.oracle_init(orc, cfg, data, b, x_init=xi)
         e = emu.instance_from_batch(cfg, data, b, x_init=xi)
         e.init(); e.associate()
-        np.testing.assert_allclose(e.field(capi.F_X), o.arr("X"), atol=1e-13)
-        np.testing.assert_allclose(e.field(capi.F_U), o.arr("U"), atol=1e-13)
         assert_association(o, e, cfg, data, b, f"instance {b}")
         assert (o.arr("U")[1, 0:3] == 0.0).all(), o.arr("U")[:, :4]   # the branch is taken: no steering while standing
