@@ -18,6 +18,8 @@ int main(int argc, char** argv)
     mpcb200_default_config(&cfg);  // unicycle, N = 20, dt_ref = 0.3, minimum_time, xf fixed, point footprint, d_min 0.5
     // solver/ipopt/max_cpu_time in seconds (default -1: no limit); a step stopped by it still succeeds (EarlyTerminated)
     if (argc > 3) cfg.max_cpu_time = std::atof(argv[3]);
+    // multistart candidates (ControllerParams::multistart_candidates, default 1: off): K > 1 also solves from K - 1 other bumped lines
+    const int multistart = argc > 4 ? std::atoi(argv[4]) : 1;
     cfg.k_max_obstacles_per_stage = 3;
     cfg.tol = 1e-8;
     std::vector<mpcb200::Obstacle> obstacles(3);
@@ -28,6 +30,7 @@ int main(int argc, char** argv)
     mpcb200::Controller controller;
     mpcb200::ControllerParams params;
     params.grid_adaptation = adapt;
+    params.multistart_candidates = multistart;
     if (!controller.configure(cfg, params, &obstacles, &via_points)) return 2;
     mpcb200::PoseSE2 x0, xf;
     xf.x = 5; xf.y = 2; xf.theta = 0;  // test_mpc_optim_node.cpp:105-106

@@ -63,6 +63,8 @@ extern "C" {
 #define MPCB200_STATUS_INVALID_INPUT 3   /* NaN/inf in the instance's inputs */
 #define MPCB200_STATUS_MAX_TIME 4        /* time budget (max_cpu_time) exhausted; the current iterate is returned (reference: Ipopt
                                             Maximum_CpuTime_Exceeded => EarlyTerminated => step() still returns true) */
+#define MPCB200_STATUS_SKIPPED 5         /* multistart challenger without an initial guess of its own (no obstacles, or start = goal
+                                            position): not solved; seen in its slot's SCAL words only, never returned */
 
 /* error codes */
 #define MPCB200_OK 0
@@ -218,6 +220,32 @@ int mpcb200_step_batch(mpcb200_handle* h, int B, const double* x0, const double*
                        double u_prev_dt, const mpcb200_obstacles* obst, const mpcb200_viapoints* vp,
                        const double* x_init, const unsigned char* reinit, double* u_seq, double* x_seq,
                        double* dt_out, int* status, double* kkt_err, int* iters, double* solve_time_s);
+
+/*
+ * mpcb200_step_batch with K candidate solves per robot in one launch; the best local optimum is returned and warm-starts the
+ * next call.  Arguments and outputs as in mpcb200_step_batch for B robots, plus:
+ *   Slots.  Candidate 0 of robot b, the incumbent, lives in slot b (the slot mpcb200_step_batch uses: the two calls share the
+ *     warm state); challenger k (1 <= k < K) lives in slot k*B + b, which this call overwrites.  B*K <= max_batch.
+ *   Initial guesses.  The incumbent starts as mpcb200_step_batch would start robot b (warm, or cold from x_init[b] or the best
+ *     bumped line).  Challenger k always starts cold from the bumped line of rank k (the 2 initial_guess_bumps + 1 lines ordered
+ *     by the cold start's score, rank 0 being the cold start's choice) and ignores x_init and reinit.  A challenger of a robot
+ *     without obstacles, or whose start and goal positions coincide, has no line of its own: it is skipped
+ *     (MPCB200_STATUS_SKIPPED in its slot) and never wins.  Challengers read robot b's inputs; nothing is copied K times.
+ *   Selection.  The converged challenger c* with the least objective (MPCB200_SC_OBJ; lower k on ties) replaces a converged
+ *     incumbent only when obj(c*) < obj(0) - (1 - hysteresis) |obj(0)|, i.e. obj(c*) < hysteresis obj(0) for obj(0) >= 0
+ *     (teb's selection_cost_hysteresis; 1: any improvement), and replaces an incumbent that did not converge always.  With no
+ *     candidate converged, an incumbent stopped by max_iter or max_cpu_time stays; failing that, the challenger stopped that way
+ *     with the least infeasibility (MPCB200_SC_INF; lower k on ties) wins; otherwise the incumbent stays.
+ *   After selection a winning challenger's state is copied into slot b, so the next call warm-starts robot b from it; the
+ *   outputs are the winner's, and winner[b] (optional) = its candidate index.  solve_time_s covers the solve and the selection;
+ *   max_cpu_time is one budget for all B*K candidates, outer_iterations applies to each.
+ * E_INVALID (nothing enqueued): K < 1, B*K > max_batch, K - 1 > 2 initial_guess_bumps, hysteresis not finite or <= 0.
+ * E_UNSUPPORTED: K > 1 with reference_initial_guess = 1 or initial_guess_bumps > 31; MPCB200_OPT_SOLVE_MODE 1.
+ */
+int mpcb200_step_batch_multistart(mpcb200_handle* h, int B, int K, double hysteresis, const double* x0, const double* xf,
+                                  const double* u_prev, double u_prev_dt, const mpcb200_obstacles* obst, const mpcb200_viapoints* vp,
+                                  const double* x_init, const unsigned char* reinit, double* u_seq, double* x_seq, double* dt_out,
+                                  int* status, double* kkt_err, int* iters, int* winner /*[B] or NULL*/, double* solve_time_s);
 
 /*
  * The same solves for a QUEUE of `total` instances (total may exceed max_batch by any factor): the handle's max_batch

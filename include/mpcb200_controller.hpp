@@ -67,6 +67,11 @@ struct ControllerParams
     int max_grid_size = 50;
     int min_grid_size = 2;   // the solver needs 3 grid points: values below 3 act as 3
     double dt_hyst_ratio = 0.1;
+    // multistart (mpcb200_step_batch_multistart with B = 1): K > 1 solves the robot's problem from its usual initial guess and
+    // from K - 1 other bumped lines in one launch and keeps the best local optimum; a challenger replaces a converged plan only
+    // when its objective is below obj - (1 - multistart_hysteresis) |obj| (teb's selection_cost_hysteresis).  1: off.
+    int multistart_candidates = 1;
+    double multistart_hysteresis = 1.0;
 };
 
 // initial state trajectory from an initial plan (Controller::generateInitialStateTrajectory, src/controller.cpp:807-857,
@@ -128,7 +133,8 @@ class Controller
         // with grid adaptation the handle is sized for the largest horizon and starts at grid_size_ref
         mpcb200_config cap = cfg;
         if (_adapt && params.max_grid_size > cap.n) cap.n = params.max_grid_size;
-        int rc = mpcb200_create(&cap, 1, device, &_h);
+        const int K = params.multistart_candidates > 1 ? params.multistart_candidates : 1;
+        int rc = mpcb200_create(&cap, K, device, &_h);
         if (rc != MPCB200_OK)
         {
             std::fprintf(stderr, "Controller::configure(): %s\n", mpcb200_last_error(nullptr));
@@ -234,8 +240,12 @@ class Controller
         const int N = _cfg.n;
         _u.assign((size_t)N * 2, 0.0); _x.assign((size_t)N * 3, 0.0);
         int status = 0, iters = 0; double dt_out = 0, kkt = 0, secs = 0;
-        const int rc = mpcb200_step_batch(_h, 1, x0, xf, _u_prev, _u_prev_dt, ocount ? &ob : nullptr, vcount ? &vp : nullptr, x_init_ptr,
-                                          &reinit, _u.data(), _x.data(), &dt_out, &status, &kkt, &iters, &secs);
+        const int K = _params.multistart_candidates;
+        const int rc = K > 1 ? mpcb200_step_batch_multistart(_h, 1, K, _params.multistart_hysteresis, x0, xf, _u_prev, _u_prev_dt,
+                                                             ocount ? &ob : nullptr, vcount ? &vp : nullptr, x_init_ptr, &reinit, _u.data(),
+                                                             _x.data(), &dt_out, &status, &kkt, &iters, nullptr, &secs)
+                             : mpcb200_step_batch(_h, 1, x0, xf, _u_prev, _u_prev_dt, ocount ? &ob : nullptr, vcount ? &vp : nullptr, x_init_ptr,
+                                                  &reinit, _u.data(), _x.data(), &dt_out, &status, &kkt, &iters, &secs);
         if (rc != MPCB200_OK)
         {
             std::fprintf(stderr, "Controller::step(): %s\n", mpcb200_last_error(_h));

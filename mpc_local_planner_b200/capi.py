@@ -26,6 +26,7 @@ OBJ_MINIMUM_TIME, OBJ_QUADRATIC_FORM, OBJ_MINIMUM_TIME_VIA_POINTS = 0, 1, 2
 FOOTPRINT_POINT, FOOTPRINT_CIRCULAR, FOOTPRINT_TWO_CIRCLES, FOOTPRINT_LINE, FOOTPRINT_POLYGON = 0, 1, 2, 3, 4
 OBST_POINT, OBST_CIRCLE, OBST_LINE = 0, 1, 2
 STATUS_CONVERGED, STATUS_MAX_ITER, STATUS_NUMERICAL_ERROR, STATUS_INVALID_INPUT, STATUS_MAX_TIME = 0, 1, 2, 3, 4
+STATUS_SKIPPED = 5   # a multistart challenger without an initial guess of its own (its slot's SCAL words only)
 E_INVALID, E_UNSUPPORTED, E_CUDA, E_NOMEM, E_NODEVICE = -1, -2, -3, -4, -5
 F_X, F_U, F_NU, F_S, F_LAM, F_KKT, F_STEP, F_SCAL, F_OBSIDX, F_OBSGIDX = range(10)
 PHASE_INIT, PHASE_ASSOCIATE, PHASE_EVAL, PHASE_KKT, PHASE_LINESEARCH = range(5)
@@ -206,6 +207,7 @@ EXPORTS = [
     "mpcb200_create_multi", "mpcb200_step_batch_multi", "mpcb200_multi_device_controls", "mpcb200_multi_fetch_controls", "mpcb200_multi_handle",
     "mpcb200_destroy_multi", "mpcb200_multi_last_error",
     "mpcb200_step_batch_async", "mpcb200_step_batch_costmap_async", "mpcb200_check_feasible_async",
+    "mpcb200_step_batch_multistart",
 ]
 
 
@@ -227,6 +229,8 @@ def load_library(path=None):
     lib.mpcb200_create.argtypes = [C.POINTER(Config), C.c_int, C.c_int, C.POINTER(vp)]
     lib.mpcb200_step_batch.argtypes = [vp, C.c_int, dp, dp, dp, C.c_double, C.POINTER(Obstacles), C.POINTER(ViaPoints),
                                        dp, ucp, dp, dp, dp, ip, dp, ip, dp]
+    lib.mpcb200_step_batch_multistart.argtypes = [vp, C.c_int, C.c_int, C.c_double, dp, dp, dp, C.c_double, C.POINTER(Obstacles),
+                                                  C.POINTER(ViaPoints), dp, ucp, dp, dp, dp, ip, dp, ip, ip, dp]
     lib.mpcb200_solve_stream.argtypes = [vp, C.c_int, dp, dp, dp, C.c_double, C.POINTER(Obstacles), C.POINTER(ViaPoints),
                                          dp, dp, dp, ip, dp, ip, dp]
     lib.mpcb200_reset.argtypes = [vp, ucp, C.c_int]
@@ -407,6 +411,26 @@ class BatchSolver:
             _dp(out["u_seq"]), _dp(out["x_seq"]), _dp(out["dt"]), _ip(out["status"]), _dp(out["kkt_err"]),
             _ip(out["iters"]), C.byref(t))
         self._check(rc, "mpcb200_step_batch")
+        out["solve_time_s"] = t.value
+        self.B = B
+        return out
+
+    def step_multistart(self, x0, xf, K, hysteresis=1.0, u_prev=None, u_prev_dt=0.0, obstacles=None, viapoints=None, x_init=None,
+                        reinit=None):
+        """step() with K candidate solves per robot (mpcb200_step_batch_multistart): the incumbent in slot b, challenger k in slot
+        k*B + b from the bumped line of rank k; the best local optimum is returned and warm-starts the next call.  Returns the
+        dict of step() plus "winner" [B] (candidate index of each robot's result)."""
+        B, x0, xf, u_prev, o, v, xi, keep = self._prep_inputs(x0, xf, u_prev, obstacles, viapoints, x_init)
+        out = self.alloc_outputs(B)
+        out["winner"] = np.empty(B, dtype=np.int32)
+        t = C.c_double(0.0)
+        ri = np.ascontiguousarray(reinit, dtype=np.uint8) if reinit is not None else None
+        rc = self.lib.mpcb200_step_batch_multistart(
+            self.h, B, int(K), float(hysteresis), _dp(x0), _dp(xf), _dp(u_prev), float(u_prev_dt), C.byref(o) if o else None,
+            C.byref(v) if v else None, _dp(xi), ri.ctypes.data_as(C.POINTER(C.c_ubyte)) if ri is not None else None,
+            _dp(out["u_seq"]), _dp(out["x_seq"]), _dp(out["dt"]), _ip(out["status"]), _dp(out["kkt_err"]), _ip(out["iters"]),
+            _ip(out["winner"]), C.byref(t))
+        self._check(rc, "mpcb200_step_batch_multistart")
         out["solve_time_s"] = t.value
         self.B = B
         return out

@@ -102,6 +102,40 @@ struct InputPtrs
 };
 struct OutputPtrs { double* u_seq; double* x_seq; double* dt; int* status; double* kkt; int* iters; double* u_packed; };
 
+// ---- multistart (mpcb200_step_batch_multistart): candidate k of robot b is instance k * B + b ----
+// A challenger (k >= 1) starts cold from the bumped line of rank k: it has none without obstacles or without a start -> goal normal
+__device__ __forceinline__ bool challenger_has_guess(const Cfg& c, const WsLayout& L, const double* W)
+{
+    double nx, ny;
+    return bump_enabled(c, L, W) && bump_normal(L, W, &nx, &ny);
+}
+// The winner among the K candidates of one robot from their SCAL words (status < 0, an unfinished solve, counts as MAX_ITER):
+// the converged challenger with the least objective (lower k on ties) replaces a converged incumbent only when
+// obj(c*) < obj(0) - (1 - hysteresis) |obj(0)|, and always one that did not converge; with none converged, the incumbent stays
+// when it ran out of iterations or time, else the challenger stopped that way with the least infeasibility wins.  Else: 0.
+// scal(k, w): word w of candidate k's SCAL words.
+template <class Scal>
+__device__ __forceinline__ int multistart_winner(const Scal& scal, int K, double hysteresis)
+{
+    auto st = [&](int k) { const double s = scal(k, MPCB200_SC_STATUS); return s < 0 ? MPCB200_STATUS_MAX_ITER : (int)s; };
+    auto stopped = [&](int k) { return st(k) == MPCB200_STATUS_MAX_ITER || st(k) == MPCB200_STATUS_MAX_TIME; };
+    int cs = -1;
+    for (int k = 1; k < K; ++k)
+        if (st(k) == MPCB200_STATUS_CONVERGED && (cs < 0 || scal(k, MPCB200_SC_OBJ) < scal(cs, MPCB200_SC_OBJ))) cs = k;
+    if (st(0) == MPCB200_STATUS_CONVERGED)
+    {
+        if (cs < 0) return 0;
+        const double o0 = scal(0, MPCB200_SC_OBJ);
+        return scal(cs, MPCB200_SC_OBJ) < o0 - (1.0 - hysteresis) * fabs(o0) ? cs : 0;
+    }
+    if (cs >= 0) return cs;
+    if (stopped(0)) return 0;
+    int best = 0;
+    for (int k = 1; k < K; ++k)
+        if (stopped(k) && (best == 0 || scal(k, MPCB200_SC_INF) < scal(best, MPCB200_SC_INF))) best = k;
+    return best;
+}
+
 // ---- scatter the compact input arrays into an instance block (inputs of instance `src`), one warp.  Returns false
 //      (warp-uniform) when an input that will be used is not finite: the instance is reported as INVALID_INPUT.  Kernels
 //      compiled without the line-obstacle paths (LINES = false) also reject a line obstacle: they would take its distance as
@@ -188,8 +222,10 @@ __device__ __forceinline__ void gather_one(const WsLayout& L, const double* W, c
 }
 
 // ---- PHASE_INIT (one warp): cold initial guess or warm-start shift ----------------------------------------
-// xinit: the instance's initial plan samples [N][3] (read when IN_HASXINIT)
-__device__ __forceinline__ void dev_init(const Cfg& c, const WsLayout& L, double* W, const ObstSrc& os, const double* xinit, int force_cold, int lane)
+// xinit: the instance's initial plan samples [N][3] (read when IN_HASXINIT); rank: the bumped line a cold start takes (0: the best,
+// k: a multistart challenger's, bump_ranked_amplitude)
+__device__ __forceinline__ void dev_init(const Cfg& c, const WsLayout& L, double* W, const ObstSrc& os, const double* xinit, int force_cold, int lane,
+                                         int rank)
 {
     const int N = L.N;
     __syncwarp();   // (see dev_kkt)
@@ -203,15 +239,11 @@ __device__ __forceinline__ void dev_init(const Cfg& c, const WsLayout& L, double
         if (bump_enabled(c, L, W) && bump_normal(L, W, &nx, &ny))
         {
             // choice of the cold initial guess: candidates one after the other, their stages spread over the lanes
-            double best = 1e300, best_a = 0.0;
-            for (int m = -c.initial_guess_bumps; m <= c.initial_guess_bumps; ++m)
-            {
-                const double A = BUMP_STEP * (double)m;
+            const double best_a = bump_ranked_amplitude(c, rank, [&](double A) {
                 double v = 0.0;
                 for (int k = lane; k < N; k += 32) v += bump_stage_violation(c, L, W, os, k, A, nx, ny);
-                const double score = 1e-3 * fabs(A) + warp_sum(v);
-                if (bump_better(score, best)) { best = score; best_a = A; }
-            }
+                return 1e-3 * fabs(A) + warp_sum(v);
+            });
             for (int k = lane; k < N; k += 32)
                 if (k >= 1 && k <= N - 2) { const double o = bump_offset(N, k, best_a); AX(0, k) += o * nx; AX(1, k) += o * ny; }
             __syncwarp();

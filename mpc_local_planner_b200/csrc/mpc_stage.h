@@ -1002,21 +1002,43 @@ HD inline double bump_heading(const WsLayout& L, const double* W, int k)
 }
 // candidate m is better than the best so far only beyond rounding noise: the order of the candidates decides exact ties
 HD inline bool bump_better(double score, double best) { return score < best - 1e-9 * (1.0 + best); }
+// Amplitude of the bumped line of rank `rank` (multistart: challenger k starts from rank k): repeated selection with bump_better
+// over the lines the earlier rounds left, lower m first, so rank 0 is the cold start's choice.  score(A): the line's score,
+// 1e-3 |A| + its clearance violation.  Ranks above 0 need 2 initial_guess_bumps + 1 <= 64 (the lines taken are a bit mask).
+template <class Score>
+HD inline double bump_ranked_amplitude(const Cfg& c, int rank, const Score& score)
+{
+    const int nb = c.initial_guess_bumps;
+    unsigned long long taken = 0ull;
+    double best_a = 0.0;
+    for (int r = 0; r <= rank; ++r)
+    {
+        double best = 1e300;
+        int best_i = -1;
+        for (int m = -nb; m <= nb; ++m)
+        {
+            if (r > 0 && ((taken >> (m + nb)) & 1ull)) continue;
+            const double A = BUMP_STEP * (double)m;
+            const double s = score(A);
+            if (bump_better(s, best)) { best = s; best_a = A; best_i = m + nb; }
+        }
+        if (best_i < 0 || r == rank) break;   // (scores that are not finite: the earlier round's line stays)
+        taken |= 1ull << best_i;
+    }
+    return best_a;
+}
 // serial form (host emulator; the CUDA kernel spreads the stages of a candidate over the lanes of the warp)
-HD inline void bump_select_serial(const Cfg& c, const WsLayout& L, double* W)
+HD inline void bump_select_serial(const Cfg& c, const WsLayout& L, double* W, int rank = 0)
 {
     const int N = L.N;
     double nx, ny;
     if (!bump_enabled(c, L, W) || !bump_normal(L, W, &nx, &ny)) return;
-    double best = 1e300, best_a = 0.0;
-    for (int m = -c.initial_guess_bumps; m <= c.initial_guess_bumps; ++m)
-    {
-        const double A = BUMP_STEP * (double)m;
+    const ObstSrc os{W + L.oOBST, W + L.oOTYPE, nullptr};
+    const double best_a = bump_ranked_amplitude(c, rank, [&](double A) {
         double score = 1e-3 * fabs(A);
-        const ObstSrc os{W + L.oOBST, W + L.oOTYPE, nullptr};
         for (int k = 1; k <= N - 2; ++k) score += bump_stage_violation(c, L, W, os, k, A, nx, ny);
-        if (bump_better(score, best)) { best = score; best_a = A; }
-    }
+        return score;
+    });
     for (int k = 1; k <= N - 2; ++k) { const double o = bump_offset(N, k, best_a); AX(0, k) += o * nx; AX(1, k) += o * ny; }
     if (bump_align_headings(c, best_a))
         for (int k = 1; k <= N - 2; ++k) AX(2, k) = bump_heading(L, W, k);

@@ -21,6 +21,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <cmath>
 #include <initializer_list>
 #include <string>
 #include <vector>
@@ -111,7 +112,7 @@ __global__ void __launch_bounds__(MAX_GROUP_WARPS * 32, 3) phase_kernel(const __
     stage_in(W, Gp, img_words, bar, 0, tid);
     switch (phase)
     {
-        case MPCB200_PHASE_INIT: if (wid == 0) dev_init(c, L, W, obstacle_source(L, W, in, inst), Gp + L.oXINIT, force_cold, lane); break;
+        case MPCB200_PHASE_INIT: if (wid == 0) dev_init(c, L, W, obstacle_source(L, W, in, inst), Gp + L.oXINIT, force_cold, lane, 0); break;
         case MPCB200_PHASE_ASSOCIATE:
             if (wid == 0)
             {
@@ -185,6 +186,7 @@ struct FusedArgs
     int total;               // instances in the queue
     int queue_mode;          // 1: a queue of cold instances without blocks (mpcb200_solve_stream)
     int force_cold;
+    int cand_stride;         // multistart kernel: instance i is candidate i / cand_stride of robot i % cand_stride, whose inputs it reads
     double uprev_dt;
     int img_words;           // resident prefix
     int* queue;              // next instance
@@ -275,7 +277,9 @@ template <int WARPS> struct FusedShape;
 template <> struct FusedShape<SMALL_GROUP_WARPS> { static constexpr int MIN_CTAS = 4; };
 template <> struct FusedShape<MAX_GROUP_WARPS> { static constexpr int MIN_CTAS = 2; };
 
-template <bool LINES, bool EXT, int WARPS, int MODEL>
+// MULTI: the multistart form (mpcb200_step_batch_multistart) -- only the prologue of an instance differs (its inputs, its bump rank);
+// a separate instantiation, so that the solve kernels of the other calls keep their registers and local memory.
+template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI>
 __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve_fused_kernel(const __grid_constant__ Cfg c, const __grid_constant__ WsLayout L, const __grid_constant__ FusedArgs a)
 {
     extern __shared__ __align__(128) unsigned char dyn_smem[];
@@ -325,6 +329,7 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
         long long t_mark = clock64();
         const long long t_begin = t_mark;
         double* Gp = a.queue_mode ? nullptr : a.ws + (int64_t)inst * L.stride;
+        const int src = MULTI ? inst % a.cand_stride : inst, rank = MULTI ? inst / a.cand_stride : 0;   // inputs, bump rank
         // ---- state: warm trajectory and scalars of the block, or a fresh cold slot ----
         if (!a.queue_mode) { stage_in(W, Gp, L.oNU, bar, parity, tid); parity ^= 1u; }
         else if (tid < MPCB200_SCAL_WORDS) W[L.oSCAL + tid] = tid == MPCB200_SC_COLD ? 1.0 : (tid == MPCB200_SC_STATUS ? -1.0 : 0.0);
@@ -332,16 +337,24 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
         // ---- inputs ----
         if (wid == 0)
         {
-            const bool ok = scatter_one<LINES>(L, W, a.in, inst, lane, nullptr);
-            if (lane == 0) { s_valid = ok; ASC(MPCB200_SC_VALID) = ok ? 1.0 : 0.0; if (!ok) mark_invalid(L, W); }
+            const bool ok = scatter_one<LINES>(L, W, a.in, src, lane, nullptr);
+            if (lane == 0)
+            {
+                s_valid = ok; ASC(MPCB200_SC_VALID) = ok ? 1.0 : 0.0; if (!ok) mark_invalid(L, W);
+                if (MULTI && ok && rank > 0)   // a challenger: the straight line bumped by its rank, whatever the incumbent's plan
+                {
+                    AIN(IN_HASXINIT) = 0.0;
+                    if (!challenger_has_guess(c, L, W)) { s_valid = 0; mark_invalid(L, W); ASC(MPCB200_SC_STATUS) = (double)MPCB200_STATUS_SKIPPED; }
+                }
+            }
         }
         __syncthreads();
         if (s_valid)
         {
             const bool long_list = a.in.obst_count && a.in.obst_max > L.M;
-            const ObstSrc os = obstacle_source(L, W, a.in, inst);
+            const ObstSrc os = obstacle_source(L, W, a.in, src);
             double* gidx = W + L.oMM;   // scratch of the KKT / line-search phases, free while the association runs
-            if (wid == 0) dev_init(c, L, W, os, a.in.x_init ? a.in.x_init + (int64_t)inst * 3 * N : nullptr, a.force_cold, lane);
+            if (wid == 0) dev_init(c, L, W, os, a.in.x_init ? a.in.x_init + (int64_t)src * 3 * N : nullptr, MULTI && rank > 0 ? 1 : a.force_cold, lane, rank);
             __syncthreads();
             TICK(MPCB200_PHASE_INIT);
             for (int oi = 0; oi < outer; ++oi)
@@ -405,6 +418,28 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
         atomicAdd(a.counters + CNT_KKT_SWEEPS, n_sweeps);
         atomicAdd(a.counters + CNT_INST, n_inst);
     }
+}
+
+// ---- kernel: multistart selection, one warp per robot: the winner among the K candidates (multistart_winner), its state into
+//      slot b (and the resident obstacles' list indices of a long list), its results into output row b ----
+__global__ void multistart_select_kernel(WsLayout L, double* ws, int B, int K, double hysteresis, int long_list, OutputPtrs o, int* winner)
+{
+    const int b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (b >= B) return;
+    double* W = ws + (int64_t)b * L.stride;
+    int w = 0;
+    if (lane == 0) w = multistart_winner([&](int k, int f) { return ws[((int64_t)k * B + b) * L.stride + L.oSCAL + f]; }, K, hysteresis);
+    w = __shfl_sync(FULLMASK, w, 0);
+    if (w > 0)
+    {
+        const double* Wc = ws + ((int64_t)w * B + b) * L.stride;
+        for (int i = lane; i < L.oSTATE_END; i += 32) W[i] = Wc[i];
+        if (long_list)
+            for (int i = lane; i < L.M; i += 32) W[L.oOGIDX + i] = Wc[L.oOGIDX + i];
+    }
+    __syncwarp();
+    gather_one(L, W, o, b, lane, 32);
+    if (lane == 0 && winner) winner[b] = w;
 }
 
 // ---- kernel: gather results into compact arrays (phased path) ----------------------------------------------------------------
@@ -517,6 +552,7 @@ struct mpcb200_handle
     int order_by_history = 1;        // MPCB200_OPT_ORDER_BY_HISTORY: batch queue longest-first by the previous solve's iteration counts
     int hist_B = 0;                  // batch size of the last batch solve whose iteration counts are in batch.iters (0: none)
     int *d_prev_iters = nullptr, *d_prev_status = nullptr, *d_order = nullptr;
+    int* d_winner = nullptr;         // [max_batch] candidate index of each robot's winner (mpcb200_step_batch_multistart)
     unsigned long long budget_ns = 0;          // max_cpu_time in ns (0: no budget)
     unsigned long long* d_origin = nullptr;    // start of the current solve launch (%globaltimer), see FusedArgs
     int sm_phase_sync = -1;          // MPCB200_OPT_SM_PHASE_SYNC: co-resident CTAs of the solve kernel enter the phases together
@@ -612,18 +648,19 @@ static cudaError_t allow_smem(K kernel) { return cudaFuncSetAttribute(kernel, cu
 // ---- the kernel variants: one table per kernel.  The variants compiled for one robot / footprint model (MODEL_UNI_POINT) exist
 //      without the line-obstacle paths only (LINES = false); a request for one with them gets the generic variant.  The fixed-dt
 //      quadratic-form key (MODEL_UNI_POINT_QF) exists for the unbordered KKT only (EXT = false). ----
-using FusedKernel = decltype(&solve_fused_kernel<false, false, SMALL_GROUP_WARPS, MODEL_GENERIC>);
-template <int WARPS>
+using FusedKernel = decltype(&solve_fused_kernel<false, false, SMALL_GROUP_WARPS, MODEL_GENERIC, false>);
+template <int WARPS, bool MULTI>
 static FusedKernel fused_shape_variant(bool lines, bool ext, int model)
 {
-    if (lines) return ext ? solve_fused_kernel<true, true, WARPS, MODEL_GENERIC> : solve_fused_kernel<true, false, WARPS, MODEL_GENERIC>;
-    if (model == MODEL_UNI_POINT_QF && !ext) return solve_fused_kernel<false, false, WARPS, MODEL_UNI_POINT_QF>;
-    if (model == MODEL_UNI_POINT) return ext ? solve_fused_kernel<false, true, WARPS, MODEL_UNI_POINT> : solve_fused_kernel<false, false, WARPS, MODEL_UNI_POINT>;
-    return ext ? solve_fused_kernel<false, true, WARPS, MODEL_GENERIC> : solve_fused_kernel<false, false, WARPS, MODEL_GENERIC>;
+    if (lines) return ext ? solve_fused_kernel<true, true, WARPS, MODEL_GENERIC, MULTI> : solve_fused_kernel<true, false, WARPS, MODEL_GENERIC, MULTI>;
+    if (model == MODEL_UNI_POINT_QF && !ext) return solve_fused_kernel<false, false, WARPS, MODEL_UNI_POINT_QF, MULTI>;
+    if (model == MODEL_UNI_POINT) return ext ? solve_fused_kernel<false, true, WARPS, MODEL_UNI_POINT, MULTI> : solve_fused_kernel<false, false, WARPS, MODEL_UNI_POINT, MULTI>;
+    return ext ? solve_fused_kernel<false, true, WARPS, MODEL_GENERIC, MULTI> : solve_fused_kernel<false, false, WARPS, MODEL_GENERIC, MULTI>;
 }
-static FusedKernel fused_variant(bool lines, bool ext, bool small, int model)
+static FusedKernel fused_variant(bool lines, bool ext, bool small, int model, bool multi)
 {
-    return small ? fused_shape_variant<SMALL_GROUP_WARPS>(lines, ext, model) : fused_shape_variant<MAX_GROUP_WARPS>(lines, ext, model);
+    if (multi) return small ? fused_shape_variant<SMALL_GROUP_WARPS, true>(lines, ext, model) : fused_shape_variant<MAX_GROUP_WARPS, true>(lines, ext, model);
+    return small ? fused_shape_variant<SMALL_GROUP_WARPS, false>(lines, ext, model) : fused_shape_variant<MAX_GROUP_WARPS, false>(lines, ext, model);
 }
 using PhaseKernel = decltype(&phase_kernel<false, MODEL_GENERIC>);
 static PhaseKernel phase_variant(bool lines, int model)
@@ -748,7 +785,7 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
         return set_err(nullptr, MPCB200_E_CUDA, m);
     }
     CKC(cudaMalloc(&h->d_nactive, 8)); CKC(cudaMalloc(&h->d_queue, 4)); CKC(cudaMalloc(&h->d_smsync, (size_t)h->num_sms * SMS_WORD_STRIDE * 8)); CKC(cudaMalloc(&h->d_prev_iters, B * 4)); CKC(cudaMalloc(&h->d_prev_status, B * 4)); CKC(cudaMalloc(&h->d_order, B * 4));
-    CKC(cudaMalloc(&h->d_origin, 8));
+    CKC(cudaMalloc(&h->d_origin, 8)); CKC(cudaMalloc(&h->d_winner, B * 4));
     CKC(cudaMalloc(&h->d_counters, CNT_BYTES)); CKC(cudaMemsetAsync(h->d_counters, 0, CNT_BYTES, h->stream));
     CKC(allow_smem(kkt_warp_kernel<false>)); CKC(allow_smem(kkt_warp_kernel<true>));
     for (const bool lines : {false, true})
@@ -756,7 +793,8 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
         {
             CKC(allow_smem(phase_variant(lines, model)));
             for (const bool ext : {false, true})
-                for (const bool small : {false, true}) CKC(allow_smem(fused_variant(lines, ext, small, model)));
+                for (const bool small : {false, true})
+                    for (const bool multi : {false, true}) CKC(allow_smem(fused_variant(lines, ext, small, model, multi)));
         }
     CKC(cudaMallocHost(&h->h_nactive, 8));
     CKC(cudaEventCreateWithFlags(&h->poll_ev[0], cudaEventDisableTiming)); CKC(cudaEventCreateWithFlags(&h->poll_ev[1], cudaEventDisableTiming));
@@ -785,7 +823,7 @@ extern "C" void mpcb200_destroy(mpcb200_handle* h)
     io_release(h->batch);
     io_release(h->queue);
     void* ptrs[] = {h->ws, h->d_nactive, h->d_queue, h->d_flush, h->d_counters, h->d_smsync, h->d_prev_iters, h->d_prev_status, h->d_order,
-                    h->d_origin, h->d_resample, h->d_cm, h->d_fz};
+                    h->d_origin, h->d_winner, h->d_resample, h->d_cm, h->d_fz};
     for (void* p : ptrs) if (p) cudaFree(p);
     if (h->h_nactive) cudaFreeHost(h->h_nactive);
     for (auto& e : h->ev) cudaEventDestroy(e);
@@ -957,10 +995,11 @@ static int scatter_to_blocks(mpcb200_handle* h, int B)
 }
 
 // ---- the solve: one launch of the persistent kernel over a queue of `total` instances ----
-static int launch_fused(mpcb200_handle* h, const IoBuffers& io, int total, int queue_mode, int force_cold)
+static int launch_fused(mpcb200_handle* h, const IoBuffers& io, int total, int queue_mode, int force_cold, int cand_stride = 0 /* multistart: B */)
 {
     FusedArgs a;
     a.ws = h->ws; a.in = io.in; a.out = io.out(); a.total = total; a.queue_mode = queue_mode; a.force_cold = force_cold; a.uprev_dt = io.uprev_dt;
+    a.cand_stride = cand_stride;
     a.img_words = image_words(h, io.in); a.queue = h->d_queue; a.counters = h->d_counters;
     a.sm_sync = nullptr; a.sm_words = 0; a.sm_gates = h->sm_phase_sync == 2 ? 2 : 3;
     a.order = nullptr;
@@ -979,7 +1018,7 @@ static int launch_fused(mpcb200_handle* h, const IoBuffers& io, int total, int q
     const size_t smem = IMG_HEAD + (size_t)a.img_words * 8;
     if (smem > MAX_IMG_SMEM) return set_err(h, MPCB200_E_UNSUPPORTED, "the instance does not fit in shared memory");
     const int threads = group_threads(h), model = kernel_model(h, io);
-    const FusedKernel kernel = fused_variant(io.has_lines, kkt_is_ext(h->cfg), threads <= SMALL_GROUP_WARPS * 32, model);
+    const FusedKernel kernel = fused_variant(io.has_lines, kkt_is_ext(h->cfg), threads <= SMALL_GROUP_WARPS * 32, model, cand_stride > 0);
     int per_sm = 0;
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
     if (per_sm < 1) return set_err(h, MPCB200_E_UNSUPPORTED, "the solve kernel does not fit on an SM with this configuration");
@@ -1085,13 +1124,27 @@ static int launch_solve_async(mpcb200_handle* h, const IoBuffers& io, int total)
     return 0;
 }
 
-// One solve between the events t0 and t1: the batch (fused or phased, by the solve mode) or the queue job (always fused).
-// Reports the device time of the solve and folds the counters of the fused kernel into the statistics.
-static int timed_launch(mpcb200_handle* h, const IoBuffers& io, int total, int queue_mode, int force_cold, double* solve_time_s)
+// the K candidates per robot of a multistart solve (mpcb200_step_batch_multistart)
+struct Multistart { int B, K; double hysteresis; };
+
+// One solve between the events t0 and t1: the batch (fused or phased, by the solve mode), a multistart batch (fused, then the
+// selection) or the queue job (always fused).  Reports the device time of the solve and folds the counters of the fused kernel
+// into the statistics.
+static int timed_launch(mpcb200_handle* h, const IoBuffers& io, int total, int queue_mode, int force_cold, double* solve_time_s,
+                        const Multistart* multi = nullptr)
 {
     CK(cudaEventRecord(h->t0, h->stream));
-    const int rc = (h->solve_mode == 1 && !queue_mode) ? solve_phased(h, total, force_cold) : launch_fused(h, io, total, queue_mode, force_cold);
+    const int rc = (h->solve_mode == 1 && !queue_mode) ? solve_phased(h, total, force_cold)
+                                                       : launch_fused(h, io, total, queue_mode, force_cold, multi ? multi->B : 0);
     if (rc) return rc;
+    if (multi)
+    {
+        const int long_list = io.in.obst_count && io.in.obst_max > h->L.M;
+        multistart_select_kernel<<<grid_for(multi->B, WARPS_PER_CTA), WARPS_PER_CTA * 32, 0, h->stream>>>(h->L, h->ws, multi->B, multi->K, multi->hysteresis,
+                                                                                                      long_list, io.out(), h->d_winner);
+        h->stats.launches_total += 1;
+        CK(cudaGetLastError());
+    }
     CK(cudaEventRecord(h->t1, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     float ms = 0.f;
@@ -1148,6 +1201,30 @@ extern "C" int mpcb200_step_batch(mpcb200_handle* h, int B, const double* x0, co
     if (h->solve_mode == 1 && (rc = scatter_to_blocks(h, B))) return rc;
     h->B = B;
     if ((rc = timed_launch(h, h->batch, B, 0, 0, solve_time_s))) return rc;
+    return fetch_outputs(h, h->batch, B, u_seq, x_seq, dt_out, status, kkt_err, iters);
+}
+
+extern "C" int mpcb200_step_batch_multistart(mpcb200_handle* h, int B, int K, double hysteresis, const double* x0, const double* xf,
+                                             const double* u_prev, double u_prev_dt, const mpcb200_obstacles* obst, const mpcb200_viapoints* vp,
+                                             const double* x_init, const unsigned char* reinit, double* u_seq, double* x_seq, double* dt_out,
+                                             int* status, double* kkt_err, int* iters, int* winner, double* solve_time_s)
+{
+    int rc = check_batch(h, B);
+    if (rc) return rc;
+    if (K < 1 || (long long)B * K > h->max_batch) return set_err(h, MPCB200_E_INVALID, "multistart: K >= 1 candidates per robot and B*K <= max_batch required");
+    if (K - 1 > 2 * h->cfg.initial_guess_bumps)
+        return set_err(h, MPCB200_E_INVALID, "multistart: K - 1 challengers need as many bumped lines besides the best (K - 1 <= 2 initial_guess_bumps)");
+    if (!std::isfinite(hysteresis) || !(hysteresis > 0.0)) return set_err(h, MPCB200_E_INVALID, "multistart: hysteresis must be finite and > 0");
+    if (K > 1 && h->cfg.reference_initial_guess)
+        return set_err(h, MPCB200_E_UNSUPPORTED, "multistart: the challengers' bumped lines are solver-side preprocessing, off with reference_initial_guess");
+    if (K > 1 && h->cfg.initial_guess_bumps > 31) return set_err(h, MPCB200_E_UNSUPPORTED, "multistart: initial_guess_bumps <= 31 with K > 1");
+    if (h->solve_mode == 1) return set_err(h, MPCB200_E_UNSUPPORTED, "multistart needs the fused solve kernel (MPCB200_OPT_SOLVE_MODE 0)");
+    CK(cudaSetDevice(h->device));
+    if ((rc = load_inputs(h, h->batch, B, x0, xf, u_prev, u_prev_dt, obst, vp, x_init, reinit))) return rc;
+    h->B = B;
+    const Multistart ms{B, K, hysteresis};
+    if ((rc = timed_launch(h, h->batch, B * K, 0, 0, solve_time_s, &ms))) return rc;
+    if (winner) { CK(cudaMemcpyAsync(winner, h->d_winner, (size_t)B * 4, cudaMemcpyDeviceToHost, h->stream)); h->stats.d2h_bytes += (long long)B * 4; }
     return fetch_outputs(h, h->batch, B, u_seq, x_seq, dt_out, status, kkt_err, iters);
 }
 
