@@ -513,6 +513,11 @@ int mpcb200_set_stream(mpcb200_handle* h, void* cuda_stream);
    fixed-dt quadratic form (MPCB200_PROBLEM_FIXED_DT_QF) the tests of the problem fields too; 1 = always the kernels that read the
    model and the problem from the configuration.  Both compute the same results bit for bit (A/B comparisons). */
 #define MPCB200_OPT_FORCE_GENERIC_MODEL 7
+/* MPCB200_OPT_CRITICAL_PLACEMENT: 1 (default) = a batch solve in history order (MPCB200_OPT_ORDER_BY_HISTORY) of at most two
+   instances per CTA of the solve kernel gives its heaviest instances -- those whose previous count exceeds 1.3 x the mean per
+   CTA -- an SM each that no other CTA of the solve shares (the batch ends with its slowest instance, and an instance alone on
+   its SM iterates faster); 0 = every CTA takes from the order as it comes.  Order of execution only. */
+#define MPCB200_OPT_CRITICAL_PLACEMENT 8
 int mpcb200_set_option(mpcb200_handle* h, int option, int value);
 /* Model key of the evaluation / line-search code of the last solve launch of this handle: MPCB200_MODEL_GENERIC (also before the
    first solve) or MPCB200_MODEL_UNI_POINT (compiled for a unicycle with a point footprint, MPCB200_OPT_FORCE_GENERIC_MODEL). */

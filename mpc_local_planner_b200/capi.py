@@ -35,6 +35,7 @@ OPT_CTAS_PER_SM = 4
 OPT_SM_PHASE_SYNC = 5
 OPT_ORDER_BY_HISTORY = 6
 OPT_FORCE_GENERIC_MODEL = 7
+OPT_CRITICAL_PLACEMENT = 8
 MODEL_GENERIC, MODEL_UNI_POINT = 0, 1
 PROBLEM_GENERIC, PROBLEM_FIXED_DT_QF = 0, 1
 ASYNC_LINE_OBSTACLES = 1

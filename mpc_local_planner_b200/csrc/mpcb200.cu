@@ -29,6 +29,7 @@
 #include "mpc_device.cuh"
 #include "mpc_costmap.cuh"
 #include "mpc_gate.h"
+#include "mpc_place.h"
 
 #define WARPS_PER_CTA 4
 #define MAX_IMG_SMEM (227 * 1024 - 2048)  // dynamic shared memory a CTA may request
@@ -197,6 +198,9 @@ struct FusedArgs
     int sm_gates;                  // 3: gates before eval, KKT and line search; 2: before KKT and line search only
     unsigned long long budget_ns;  // time budget of the launch (max_cpu_time), 0: none
     unsigned long long* origin;    // %globaltimer at the start of the launch: the first CTA sets it (zeroed before the launch)
+    int* place;                    // critical placement (nullptr: off): [0] heavy instances H, [1] heavy claims (mpc_place.h)
+    unsigned long long* place_sm;  // admission word of each SM (sm_words of them): word 1 of its phase-alignment line
+    int place_cotenants;           // CTAs a heavy instance shares its SM with, at most
 };
 // ---- phase alignment of the CTAs that share an SM ---------------------------------------------------------------------------
 // The solve kernel's iteration is ~128 KB of straight fp64 code, several times an SM's instruction cache: CTAs that sit on the
@@ -206,10 +210,20 @@ struct FusedArgs
 // Timing only -- no data crosses CTAs.
 #define SMS_POLL_NS 128   // pause between two polls of the barrier word (the polling thread shares its scheduler with working warps)
 #define SMS_WORD_STRIDE 16   // words: one 128-byte line per SM
+// Critical placement (mpc_place.h; DESIGN.md 4, measured on an H100): the heavy part is the instances whose predicted count exceeds
+// PLACE_RHO x the mean per CTA slot, and each shares its SM with at most PLACE_COTENANTS other CTAs (compile-time, so that
+// tools/placement_sweep.py can compare settings as libraries of their own).
+#ifndef PLACE_RHO
+#define PLACE_RHO 1.3
+#endif
+#ifndef PLACE_COTENANTS
+#define PLACE_COTENANTS 0
+#endif
 struct DevAtomics
 {
     typedef unsigned long long Word;
     static __device__ __forceinline__ Word add(Word* w, Word v) { return atomicAdd(w, v); }
+    static __device__ __forceinline__ int add(int* w, int v) { return atomicAdd(w, v); }
     static __device__ __forceinline__ Word cas(Word* w, Word expected, Word desired) { return atomicCAS(w, expected, desired); }
     // relaxed, not acquire: no data crosses CTAs, and on sm_90a an acquire load is followed by an invalidation of the whole L1
     // (CCTL.IVALL), so every poll would throw away the cached global data of the CTAs that share the SM
@@ -230,16 +244,22 @@ __device__ __forceinline__ unsigned sm_index() { unsigned r; asm volatile("mov.u
 // hard in this one, so the history is the hint.  Counting sort (descending, stable) by min(iters, 1023) in one CTA.
 // An instance the time budget stopped (MPCB200_STATUS_MAX_TIME) counts as needing max_iter iterations whatever it ran: otherwise
 // the instances the queue never reached (iters 0) would go last again and stay unsolved in every cycle.
+// With the critical placement (place != nullptr) the kernel also plans the heavy part of mpc_place.h: the H leading instances whose
+// count exceeds rho x the mean count per CTA slot (the batch's total over `slots`), at most max_heavy; it writes H and a zero
+// claim count to place[0..1] and starts the queue counter (the light part) at H.
 __device__ __forceinline__ int history_key(const int* prev_iters, const int* prev_status, int max_iter, int i)
 {
     const int k = prev_status[i] == MPCB200_STATUS_MAX_TIME ? max_iter : prev_iters[i];
     return k < 0 ? 0 : (k > 1023 ? 1023 : k);
 }
 __global__ void __launch_bounds__(1024) order_by_history_kernel(const int* __restrict__ prev_iters, const int* __restrict__ prev_status, int max_iter,
-                                                                int B, int* __restrict__ order)
+                                                                int B, int* __restrict__ order, int* place, int slots, double rho,
+                                                                int max_heavy, int* queue)
 {
     __shared__ int hist[1024];
     __shared__ int warp_tot[32];
+    __shared__ unsigned long long s_work;
+    __shared__ int s_heavy;
     const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
     hist[t] = 0;
     __syncthreads();
@@ -247,6 +267,16 @@ __global__ void __launch_bounds__(1024) order_by_history_kernel(const int* __res
     __syncthreads();
     // exclusive scan of hist (bucket 0 = the longest)
     const int v = hist[t];
+    if (place)
+    {
+        if (t == 0) { s_work = 0ull; s_heavy = 0; }
+        __syncthreads();
+        atomicAdd(&s_work, (unsigned long long)v * (unsigned long long)(1023 - t));
+        __syncthreads();
+        if (v > 0 && (double)(1023 - t) > rho * (double)s_work / (double)slots) atomicAdd(&s_heavy, v);
+        __syncthreads();
+        if (t == 0) { const int H = s_heavy < max_heavy ? s_heavy : max_heavy; place[0] = H; place[1] = 0; *queue = H; }
+    }
     int incl = v;
     for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(FULLMASK, incl, o); if (lane >= o) incl += u; }
     if (lane == 31) warp_tot[wid] = incl;
@@ -284,7 +314,7 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
 {
     extern __shared__ __align__(128) unsigned char dyn_smem[];
     __shared__ CtaShared sh;
-    __shared__ int s_inst, s_valid, s_solo;
+    __shared__ int s_inst, s_valid, s_solo, s_next;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nt = blockDim.x;
     const int N = L.N;
     double* W = reinterpret_cast<double*>(dyn_smem + IMG_HEAD);
@@ -302,6 +332,7 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
         }
         sh.deadline = deadline;
         s_solo = 0;
+        s_next = place::ADMIT;
     }
     CudaWarp<EXT> ex;
     ex.lane = lane;
@@ -322,7 +353,26 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
 #define TICK(p_) do { const long long t_ = clock64(); cyc[p_] += (unsigned long long)(t_ - t_mark); t_mark = t_; } while (0)
     for (;;)
     {
-        if (tid == 0) { const int q = atomicAdd(a.queue, 1); s_inst = (q < a.total && a.order) ? a.order[q] : q; }
+        if (tid == 0)
+        {
+            if (!a.place) { const int q = atomicAdd(a.queue, 1); s_inst = (q < a.total && a.order) ? a.order[q] : q; }
+            else
+            {
+                int nx = s_next;   // (admission here rather than in the prologue: it leaves every variant's registers and spills alone)
+                if (nx == place::ADMIT)
+                {
+                    nx = place::TAKE;
+                    const unsigned smid = sm_index();
+                    if (smid < (unsigned)a.sm_words)
+                    {
+                        nx = place::admit<DevAtomics>(a.place_sm + (size_t)smid * SMS_WORD_STRIDE, a.place, a.order, (unsigned)a.place_cotenants);
+                        s_solo = nx >= 0 && a.place_cotenants == 0;   // a heavy instance alone on its SM: no gates
+                    }
+                }
+                s_next = place::TAKE;
+                s_inst = nx >= 0 ? nx : (nx == place::LEAVE ? a.total : place::take<DevAtomics>(a.queue, a.place, a.order, a.total));
+            }
+        }
         __syncthreads();
         const int inst = s_inst;
         if (inst >= a.total) break;
@@ -550,6 +600,7 @@ struct mpcb200_handle
     double* d_flush = nullptr; size_t flush_n = 0;
     int fused_grid = 0;              // CTAs of the last fused launch
     int order_by_history = 1;        // MPCB200_OPT_ORDER_BY_HISTORY: batch queue longest-first by the previous solve's iteration counts
+    int critical_placement = 1;      // MPCB200_OPT_CRITICAL_PLACEMENT: the heaviest instances of a history order get SMs of their own
     int hist_B = 0;                  // batch size of the last batch solve whose iteration counts are in batch.iters (0: none)
     int *d_prev_iters = nullptr, *d_prev_status = nullptr, *d_order = nullptr;
     int* d_winner = nullptr;         // [max_batch] candidate index of each robot's winner (mpcb200_step_batch_multistart)
@@ -784,7 +835,7 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
         mpcb200_destroy(h);
         return set_err(nullptr, MPCB200_E_CUDA, m);
     }
-    CKC(cudaMalloc(&h->d_nactive, 8)); CKC(cudaMalloc(&h->d_queue, 4)); CKC(cudaMalloc(&h->d_smsync, (size_t)h->num_sms * SMS_WORD_STRIDE * 8)); CKC(cudaMalloc(&h->d_prev_iters, B * 4)); CKC(cudaMalloc(&h->d_prev_status, B * 4)); CKC(cudaMalloc(&h->d_order, B * 4));
+    CKC(cudaMalloc(&h->d_nactive, 8)); CKC(cudaMalloc(&h->d_queue, 4)); CKC(cudaMalloc(&h->d_smsync, (size_t)h->num_sms * SMS_WORD_STRIDE * 8)); CKC(cudaMalloc(&h->d_prev_iters, B * 4)); CKC(cudaMalloc(&h->d_prev_status, B * 4)); CKC(cudaMalloc(&h->d_order, (B + 2) * 4));
     CKC(cudaMalloc(&h->d_origin, 8)); CKC(cudaMalloc(&h->d_winner, B * 4));
     CKC(cudaMalloc(&h->d_counters, CNT_BYTES)); CKC(cudaMemsetAsync(h->d_counters, 0, CNT_BYTES, h->stream));
     CKC(allow_smem(kkt_warp_kernel<false>)); CKC(allow_smem(kkt_warp_kernel<true>));
@@ -1002,19 +1053,9 @@ static int launch_fused(mpcb200_handle* h, const IoBuffers& io, int total, int q
     a.cand_stride = cand_stride;
     a.img_words = image_words(h, io.in); a.queue = h->d_queue; a.counters = h->d_counters;
     a.sm_sync = nullptr; a.sm_words = 0; a.sm_gates = h->sm_phase_sync == 2 ? 2 : 3;
-    a.order = nullptr;
+    a.order = nullptr; a.place = nullptr; a.place_sm = nullptr; a.place_cotenants = PLACE_COTENANTS;
     a.budget_ns = h->budget_ns; a.origin = h->d_origin;
     if (h->budget_ns) CK(cudaMemsetAsync(h->d_origin, 0, 8, h->stream));
-    if (!queue_mode && h->order_by_history && h->hist_B == total && total > h->num_sms)
-    {
-        // (the iteration counts and statuses are rewritten by this solve: order from copies)
-        CK(cudaMemcpyAsync(h->d_prev_iters, io.iters, (size_t)total * 4, cudaMemcpyDeviceToDevice, h->stream));
-        CK(cudaMemcpyAsync(h->d_prev_status, io.status, (size_t)total * 4, cudaMemcpyDeviceToDevice, h->stream));
-        order_by_history_kernel<<<1, 1024, 0, h->stream>>>(h->d_prev_iters, h->d_prev_status, h->cfg.max_iter, total, h->d_order);
-        h->stats.launches_total += 1;
-        a.order = h->d_order;
-    }
-    if (!queue_mode) h->hist_B = total;
     const size_t smem = IMG_HEAD + (size_t)a.img_words * 8;
     if (smem > MAX_IMG_SMEM) return set_err(h, MPCB200_E_UNSUPPORTED, "the instance does not fit in shared memory");
     const int threads = group_threads(h), model = kernel_model(h, io);
@@ -1025,13 +1066,26 @@ static int launch_fused(mpcb200_handle* h, const IoBuffers& io, int total, int q
     if (h->max_ctas_per_sm > 0 && per_sm > h->max_ctas_per_sm) per_sm = h->max_ctas_per_sm;
     const int grid = total < per_sm * h->num_sms ? total : per_sm * h->num_sms;
     h->fused_grid = grid;
-    // phase alignment pays when several CTAs share an SM (auto: from three CTAs per SM)
-    if (h->sm_phase_sync > 0 || (h->sm_phase_sync < 0 && per_sm >= 3 && grid > h->num_sms))
-    {
-        a.sm_sync = h->d_smsync; a.sm_words = h->num_sms;
-        CK(cudaMemsetAsync(h->d_smsync, 0, (size_t)h->num_sms * SMS_WORD_STRIDE * 8, h->stream));
-    }
     CK(cudaMemsetAsync(h->d_queue, 0, 4, h->stream));
+    if (!queue_mode && h->order_by_history && h->hist_B == total && total > h->num_sms)
+    {
+        // The critical placement needs SMs that a heavy instance could share, and a batch of at most two instances per CTA slot:
+        // with more, the heavy part is empty or nearly so (its threshold is 1.3 x the mean count per slot), and the placed
+        // launch measured 2-3 % slower there (cfg 4 at B = 16 384, cfg 5 at B = 2048; H100, DESIGN.md 4).
+        const bool placing = h->critical_placement && per_sm >= 2 && total <= 2 * grid;
+        if (placing) { a.place = h->d_order + total; a.place_sm = h->d_smsync + 1; a.sm_words = h->num_sms; }
+        // (the iteration counts and statuses are rewritten by this solve: order from copies)
+        CK(cudaMemcpyAsync(h->d_prev_iters, io.iters, (size_t)total * 4, cudaMemcpyDeviceToDevice, h->stream));
+        CK(cudaMemcpyAsync(h->d_prev_status, io.status, (size_t)total * 4, cudaMemcpyDeviceToDevice, h->stream));
+        order_by_history_kernel<<<1, 1024, 0, h->stream>>>(h->d_prev_iters, h->d_prev_status, h->cfg.max_iter, total, h->d_order,
+                                                            a.place, grid, PLACE_RHO, h->num_sms, h->d_queue);
+        h->stats.launches_total += 1;
+        a.order = h->d_order;
+    }
+    if (!queue_mode) h->hist_B = total;
+    // phase alignment pays when several CTAs share an SM (auto: from three CTAs per SM)
+    if (h->sm_phase_sync > 0 || (h->sm_phase_sync < 0 && per_sm >= 3 && grid > h->num_sms)) { a.sm_sync = h->d_smsync; a.sm_words = h->num_sms; }
+    if (a.sm_sync || a.place) CK(cudaMemsetAsync(h->d_smsync, 0, (size_t)h->num_sms * SMS_WORD_STRIDE * 8, h->stream));
     kernel<<<grid, threads, smem, h->stream>>>(h->cfg, h->L, a);
     h->last_model = model;
     h->stats.launches_total += 1;
@@ -1423,6 +1477,7 @@ extern "C" int mpcb200_set_option(mpcb200_handle* h, int option, int value)
     if (option == MPCB200_OPT_ORDER_BY_HISTORY && value >= 0 && value <= 1) { h->order_by_history = value; return 0; }
     if (option == MPCB200_OPT_SM_PHASE_SYNC && value >= -1 && value <= 2) { h->sm_phase_sync = value; return 0; }
     if (option == MPCB200_OPT_FORCE_GENERIC_MODEL && value >= 0 && value <= 1) { h->force_generic_model = value; return 0; }
+    if (option == MPCB200_OPT_CRITICAL_PLACEMENT && value >= 0 && value <= 1) { h->critical_placement = value; return 0; }
     return set_err(h, MPCB200_E_INVALID, "unknown option or value");
 }
 

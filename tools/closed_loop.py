@@ -2,7 +2,7 @@
 from the previous solution (shifted on the device), applies the first control for the cycle time with the exact unicycle
 flow, and feeds the new state and the applied control back -- the steady state `MpcLocalPlannerROS::computeVelocityCommands`
 runs in.  Prints per-cycle device time, iterations and the fraction of robots whose solve converged.
-Usage: python tools/closed_loop.py [B] [cycles]"""
+Usage: python tools/closed_loop.py [B] [cycles] [critical placement 0|1 (default: the library's, MPCB200_OPT_CRITICAL_PLACEMENT)]"""
 import sys; sys.path.insert(0, '.')
 import numpy as np
 from mpc_local_planner_b200 import capi, configs
@@ -13,6 +13,8 @@ T = 0.2  # control period (5 Hz, EX/launch/diff_drive_quadratic_form.launch:37)
 cfg = configs.config_for(2, tol=1e-6)
 data = configs.generate(2, B)
 s = capi.BatchSolver(cfg, B)
+if len(sys.argv) > 3:
+    s.set_option(capi.OPT_CRITICAL_PLACEMENT, int(sys.argv[3]))
 x = data["x0"].copy(); u_prev = data["u_prev"].copy()
 alive = np.ones(B, bool)
 rows = []
