@@ -20,6 +20,8 @@ int main(int argc, char** argv)
     if (argc > 3) cfg.max_cpu_time = std::atof(argv[3]);
     // multistart candidates (ControllerParams::multistart_candidates, default 1: off): K > 1 also solves from K - 1 other bumped lines
     const int multistart = argc > 4 ? std::atoi(argv[4]) : 1;
+    // robot/unicycle/max_vel_x from the second step on (Controller::setRobotLimits; default: the configuration's 0.4 throughout)
+    const double max_vel_x = argc > 5 ? std::atof(argv[5]) : 0.0;
     cfg.k_max_obstacles_per_stage = 3;
     cfg.tol = 1e-8;
     std::vector<mpcb200::Obstacle> obstacles(3);
@@ -37,6 +39,12 @@ int main(int argc, char** argv)
     mpcb200::TimeSeries u_seq, x_seq;
     for (int i = 0; i < steps; ++i)
     {
+        if (i == 1 && max_vel_x > 0)   // a speed-limit zone from the second step on: max_vel_x lowered, the other limits kept
+        {
+            double limits[MPCB200_LIMIT_WORDS] = {cfg.u_lb[0], cfg.u_lb[1], max_vel_x, cfg.u_ub[1], cfg.du_lb[0], cfg.du_lb[1],
+                                                  cfg.du_ub[0], cfg.du_ub[1], cfg.min_obstacle_dist};
+            if (!controller.setRobotLimits(limits)) return 2;
+        }
         const bool ok = controller.step(x0, xf, mpcb200::Twist(), 0.05, 0.05 * i, &u_seq, &x_seq);
         const int n = controller.gridSize();
         std::printf("step %d ok %d status %d iters %d dt %.9f u0 %.9f %.9f xN %.6f %.6f %.6f kkt %.2e n %d\n", i, (int)ok, controller.lastStatus(),

@@ -248,6 +248,46 @@ int mpcb200_step_batch_multistart(mpcb200_handle* h, int B, int K, double hyster
                                   int* status, double* kkt_err, int* iters, int* winner /*[B] or NULL*/, double* solve_time_s);
 
 /*
+ * Per-robot limits: robots with different speed, acceleration and clearance limits in one handle and one solve launch (the
+ * reference's per-Controller robot/<type>/max_vel_x, max_vel_x_backwards, max_vel_theta | max_steering_angle, src/controller.cpp:
+ * 496-541; acc_lim_* / dec_lim_* / max_steering_rate, :735-791; collision_avoidance/min_obstacle_dist, :717-728).  A record is
+ * MPCB200_LIMIT_WORDS doubles:
+ *   [MPCB200_LIM_U_LB + i]   u_lb[i]     [MPCB200_LIM_U_UB + i]   u_ub[i]      (i = 0, 1)
+ *   [MPCB200_LIM_DU_LB + i]  du_lb[i]    [MPCB200_LIM_DU_UB + i]  du_ub[i]
+ *   [MPCB200_LIM_MIN_OBSTACLE_DIST]      min_obstacle_dist
+ *   Scope.  Once set, record b applies to robot b of every later solve call of the handle until it is replaced or cleared:
+ *     mpcb200_step_batch, _step_batch_async, _step_batch_costmap, _step_batch_costmap_async, _solve_resident and
+ *     _step_batch_multistart (the K candidates of robot b all use record b).  mpcb200_reset and mpcb200_resample keep the records.
+ *   Values.  The record's values are used wherever the configuration's are read, and nowhere else: the bound and control-rate
+ *     rows of the evaluation and the line search, the cold start's control seeding, and the clearance of the bumped-line scoring,
+ *     the pose repair and the obstacle rows.  A robot whose record changed between two calls warm-starts from its previous
+ *     solution under the new values.  Which rows exist stays a property of the handle: a bound that is finite in the
+ *     configuration must be finite in every record, and one that is off (|bound| >= MPCB200_INF) must be off.  The kernel key
+ *     (mpcb200_kernel_model / _problem) is the same with and without records.
+ *   Validity (mpc_core.h robot_limits_valid): no word is NaN, u_ub[i] > u_lb[i], every bound finite exactly where the
+ *     configuration's is, and 0 <= min_obstacle_dist < inf.
+ *   mpcb200_set_robot_limits: `limits` = host [n][MPCB200_LIMIT_WORDS]; n = 0 clears (limits may be NULL).  E_INVALID, and nothing
+ *     changes, when n < 0 or n > max_batch, limits is NULL with n > 0, or a record is not valid.
+ *   mpcb200_set_robot_limits_async: `limits` = device [n][MPCB200_LIMIT_WORDS] of the handle's device, copied device to device on
+ *     the handle's stream into an array allocated at create for max_batch records (capturable in a CUDA graph); the host reads no
+ *     record.  The solve checks each robot's record instead: a robot whose record is not valid gets MPCB200_STATUS_INVALID_INPUT
+ *     and is not iterated; the other robots are unaffected.  n = 0 clears.
+ *   While records are set: a solve call with more robots than records returns E_INVALID and enqueues nothing;
+ *     mpcb200_solve_stream (queue entries are not robots), MPCB200_OPT_SOLVE_MODE 1 and mpcb200_run_phase / mpcb200_time_phase
+ *     return E_UNSUPPORTED.
+ *   Several devices (mpcb200_create_multi): the records are set per device handle (mpcb200_multi_handle), record b of rank r for
+ *     the b-th robot of that device's block of the batch.
+ */
+#define MPCB200_LIMIT_WORDS 9
+#define MPCB200_LIM_U_LB 0
+#define MPCB200_LIM_U_UB 2
+#define MPCB200_LIM_DU_LB 4
+#define MPCB200_LIM_DU_UB 6
+#define MPCB200_LIM_MIN_OBSTACLE_DIST 8
+int mpcb200_set_robot_limits(mpcb200_handle* h, int n, const double* limits);
+int mpcb200_set_robot_limits_async(mpcb200_handle* h, int n, const double* limits);
+
+/*
  * The same solves for a QUEUE of `total` instances (total may exceed max_batch by any factor): the handle's max_batch
  * workspaces form a pool of slots, and a slot whose instance has finished hands its result over and takes the next
  * instance of the queue while the other slots keep iterating (continuous batching).  The interior-point iterations of

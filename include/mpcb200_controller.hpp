@@ -142,8 +142,31 @@ class Controller
             return false;
         }
         if (!setHorizon(_n_ref)) return false;
+        if (_has_limits && !applyRobotLimits()) return false;
         _ocp_seq = 0; _grid_empty = true; _ocp_successful = false;
         return true;
+    }
+
+    // Runtime limits of this robot (mpcb200_set_robot_limits with one record): u_lb[2], u_ub[2], du_lb[2], du_ub[2] and
+    // min_obstacle_dist in place of the configuration's (a speed-limit zone, a payload, people nearby); with multistart they
+    // cover all its candidates.  The next step warm-starts under the new values.  They survive reset(), grid adaptation and a
+    // new configure(); false (and the previous limits kept) when the record is not valid for the configuration (mpcb200.h).
+    bool setRobotLimits(const double limits[MPCB200_LIMIT_WORDS])
+    {
+        if (_h && mpcb200_set_robot_limits(_h, 1, limits) != MPCB200_OK)
+        {
+            std::fprintf(stderr, "Controller::setRobotLimits(): %s\n", mpcb200_last_error(_h));
+            return false;
+        }
+        for (int i = 0; i < MPCB200_LIMIT_WORDS; ++i) _limits[i] = limits[i];
+        _has_limits = true;
+        return true;
+    }
+    // back to the configuration's limits
+    void clearRobotLimits()
+    {
+        if (_h) mpcb200_set_robot_limits(_h, 0, nullptr);
+        _has_limits = false;
     }
 
     // StructuredOptimalControlProblem::setPreviousControlInput (called by the planner before step, src/mpc_local_planner_ros.cpp:384)
@@ -299,6 +322,12 @@ class Controller
         _cfg.n = n;
         return true;
     }
+    bool applyRobotLimits()
+    {
+        if (mpcb200_set_robot_limits(_h, 1, _limits) == MPCB200_OK) return true;
+        std::fprintf(stderr, "Controller: robot limits: %s\n", mpcb200_last_error(_h));
+        return false;
+    }
     static void fill(TimeSeries& ts, const std::vector<double>& v, int dim, int N, double dt)
     {
         ts.clear(); ts.dim = dim;
@@ -320,6 +349,8 @@ class Controller
     bool _grid_empty = true, _ocp_successful = false;
     double _last_dt = 0, _last_kkt = 0, _last_solve_time = 0;
     int _last_status = -1, _last_iters = 0;
+    double _limits[MPCB200_LIMIT_WORDS] = {};
+    bool _has_limits = false;   // setRobotLimits in effect
 };
 
 }  // namespace mpcb200

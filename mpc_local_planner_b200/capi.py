@@ -39,6 +39,9 @@ OPT_CRITICAL_PLACEMENT = 8
 MODEL_GENERIC, MODEL_UNI_POINT = 0, 1
 PROBLEM_GENERIC, PROBLEM_FIXED_DT_QF = 0, 1
 ASYNC_LINE_OBSTACLES = 1
+# per-robot limits (mpcb200_set_robot_limits): words of a record
+LIMIT_WORDS = 9
+LIM_U_LB, LIM_U_UB, LIM_DU_LB, LIM_DU_UB, LIM_MIN_OBSTACLE_DIST = 0, 2, 4, 6, 8
 SOLVE_FUSED, SOLVE_PHASED = 0, 1
 NUM_PHASES = 5
 K_H, K_G, K_A, K_B, K_E, K_C, K_HB, K_D = 0, 15, 20, 23, 29, 32, 34, 39
@@ -209,6 +212,7 @@ EXPORTS = [
     "mpcb200_destroy_multi", "mpcb200_multi_last_error",
     "mpcb200_step_batch_async", "mpcb200_step_batch_costmap_async", "mpcb200_check_feasible_async",
     "mpcb200_step_batch_multistart",
+    "mpcb200_set_robot_limits", "mpcb200_set_robot_limits_async",
 ]
 
 
@@ -232,6 +236,8 @@ def load_library(path=None):
                                        dp, ucp, dp, dp, dp, ip, dp, ip, dp]
     lib.mpcb200_step_batch_multistart.argtypes = [vp, C.c_int, C.c_int, C.c_double, dp, dp, dp, C.c_double, C.POINTER(Obstacles),
                                                   C.POINTER(ViaPoints), dp, ucp, dp, dp, dp, ip, dp, ip, ip, dp]
+    lib.mpcb200_set_robot_limits.argtypes = [vp, C.c_int, dp]
+    lib.mpcb200_set_robot_limits_async.argtypes = [vp, C.c_int, vp]
     lib.mpcb200_solve_stream.argtypes = [vp, C.c_int, dp, dp, dp, C.c_double, C.POINTER(Obstacles), C.POINTER(ViaPoints),
                                          dp, dp, dp, ip, dp, ip, dp]
     lib.mpcb200_reset.argtypes = [vp, ucp, C.c_int]
@@ -435,6 +441,28 @@ class BatchSolver:
         out["solve_time_s"] = t.value
         self.B = B
         return out
+
+    def set_robot_limits(self, a):
+        """Per-robot limits (mpcb200_set_robot_limits): a = [n, LIMIT_WORDS] (u_lb[2], u_ub[2], du_lb[2], du_ub[2],
+        min_obstacle_dist per robot) replaces those config values for robots 0..n-1 of every later solve; None clears."""
+        if a is None:
+            self._check(self.lib.mpcb200_set_robot_limits(self.h, 0, None), "mpcb200_set_robot_limits")
+            return
+        a = np.ascontiguousarray(a, dtype=np.float64)
+        if a.ndim != 2 or a.shape[1] != LIMIT_WORDS:
+            raise ValueError(f"limits must have shape [n, {LIMIT_WORDS}], got {a.shape}")
+        self._check(self.lib.mpcb200_set_robot_limits(self.h, a.shape[0], _dp(a)), "mpcb200_set_robot_limits")
+
+    def set_robot_limits_async(self, t):
+        """set_robot_limits() from a torch CUDA tensor float64 [n, LIMIT_WORDS] (mpcb200_set_robot_limits_async): copied on the
+        handle's stream, which must be torch's current stream; the solve checks each robot's record (an invalid one makes its
+        robot STATUS_INVALID_INPUT).  None clears."""
+        torch = self._async_prologue()
+        if t is None:
+            self._check(self.lib.mpcb200_set_robot_limits_async(self.h, 0, None), "mpcb200_set_robot_limits_async")
+            return
+        p = _tensor_ptr(t, "limits", torch.float64, self.device, (None, LIMIT_WORDS))
+        self._check(self.lib.mpcb200_set_robot_limits_async(self.h, int(t.shape[0]), p), "mpcb200_set_robot_limits_async")
 
     def upload(self, x0, xf, u_prev=None, u_prev_dt=0.0, obstacles=None, viapoints=None, x_init=None):
         B, x0, xf, u_prev, o, v, xi, keep = self._prep_inputs(x0, xf, u_prev, obstacles, viapoints, x_init)

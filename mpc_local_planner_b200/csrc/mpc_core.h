@@ -119,6 +119,39 @@ HD inline bool control_row_finite(const Cfg& c, int slot)
     return ((slot - 4) & 1) ? (c.du_ub[i] < MPCB200_INF) : (c.du_lb[i] > -MPCB200_INF);
 }
 
+// ---- per-robot limits (mpcb200_set_robot_limits): a record of MPCB200_LIMIT_WORDS doubles in place of nine config values ----
+// A record may change values, never the row set: each of the eight control rows is finite in the record exactly where it is in
+// `c` (the kernel variant and the fixed-dt key are chosen from `c`), the rule of mpcb200_create (u_ub > u_lb) holds, no word is
+// NaN and the clearance is finite and >= 0.  The blocking setter checks every record with this on the host, the solve kernel
+// checks the record of each robot with it in the instance's prologue.
+HD inline bool robot_limits_valid(const Cfg& c, const double* r)
+{
+    for (int w = 0; w < MPCB200_LIMIT_WORDS; ++w)
+        if (r[w] != r[w]) return false;
+    for (int i = 0; i < 2; ++i)
+    {
+        if (!(r[MPCB200_LIM_U_UB + i] > r[MPCB200_LIM_U_LB + i])) return false;
+        if ((r[MPCB200_LIM_U_LB + i] > -MPCB200_INF) != control_row_finite(c, 2 * i)) return false;
+        if ((r[MPCB200_LIM_U_UB + i] < MPCB200_INF) != control_row_finite(c, 2 * i + 1)) return false;
+        if ((r[MPCB200_LIM_DU_LB + i] > -MPCB200_INF) != control_row_finite(c, 4 + 2 * i)) return false;
+        if ((r[MPCB200_LIM_DU_UB + i] < MPCB200_INF) != control_row_finite(c, 5 + 2 * i)) return false;
+    }
+    const double d = r[MPCB200_LIM_MIN_OBSTACLE_DIST];
+    return d >= 0.0 && d <= 1.7976931348623157e308;
+}
+// the configuration of a robot: its record's nine values in place of the configuration's, every other field untouched
+HD inline void apply_robot_limits(Cfg& c, const double* r)
+{
+    for (int i = 0; i < 2; ++i)
+    {
+        c.u_lb[i] = r[MPCB200_LIM_U_LB + i];
+        c.u_ub[i] = r[MPCB200_LIM_U_UB + i];
+        c.du_lb[i] = r[MPCB200_LIM_DU_LB + i];
+        c.du_ub[i] = r[MPCB200_LIM_DU_UB + i];
+    }
+    c.min_obstacle_dist = r[MPCB200_LIM_MIN_OBSTACLE_DIST];
+}
+
 // ---- model / problem key of a kernel variant ----
 // MODEL_GENERIC reads the robot and footprint model from the configuration at run time.  MODEL_UNI_POINT is compiled for the
 // unicycle with a point footprint (the BASELINE configurations 2, 4 and 5): the tests of the two fields fold at compile time and the

@@ -307,11 +307,23 @@ template <int WARPS> struct FusedShape;
 template <> struct FusedShape<SMALL_GROUP_WARPS> { static constexpr int MIN_CTAS = 4; };
 template <> struct FusedShape<MAX_GROUP_WARPS> { static constexpr int MIN_CTAS = 2; };
 
-// MULTI: the multistart form (mpcb200_step_batch_multistart) -- only the prologue of an instance differs (its inputs, its bump rank);
-// a separate instantiation, so that the solve kernels of the other calls keep their registers and local memory.
-template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI>
-__global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve_fused_kernel(const __grid_constant__ Cfg c, const __grid_constant__ WsLayout L, const __grid_constant__ FusedArgs a)
+// Per-robot limits (mpcb200_set_robot_limits): the records, and one configuration per CTA in global memory -- the handle's
+// configuration with the record of the CTA's current instance applied.  (A copy in shared memory would cost cfg 2 one of its
+// four CTAs per SM: 848 bytes more than the 56 KB images leave.)
+struct RobotArgs
 {
+    const double* limits;   // [robots][MPCB200_LIMIT_WORDS]
+    Cfg* cfg;               // [grid] the configuration CTA blockIdx.x presents to the phases
+};
+
+// The solve of the persistent kernel.  c0 is the handle's configuration.  MULTI: the multistart form (mpcb200_step_batch_multistart);
+// ROBOT: the per-robot-limits form.  Either only changes the prologue of an instance (MULTI: its inputs, its bump rank; ROBOT: the
+// configuration the phases read), and each is an instantiation of its own, so that the solve kernels of the other calls keep their
+// registers and local memory.
+template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI, bool ROBOT>
+__device__ __forceinline__ void solve_fused(const Cfg& c0, const WsLayout& L, const FusedArgs& a, const RobotArgs& r)
+{
+    const Cfg& c = ROBOT ? r.cfg[blockIdx.x] : c0;
     extern __shared__ __align__(128) unsigned char dyn_smem[];
     __shared__ CtaShared sh;
     __shared__ int s_inst, s_valid, s_solo, s_next;
@@ -334,9 +346,15 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
         s_solo = 0;
         s_next = place::ADMIT;
     }
+    if (ROBOT)
+    {
+        const unsigned long long* src = reinterpret_cast<const unsigned long long*>(&c0);
+        unsigned long long* dst = reinterpret_cast<unsigned long long*>(r.cfg + blockIdx.x);
+        for (int i = tid; i < (int)(sizeof(Cfg) / 8); i += nt) dst[i] = src[i];
+    }
     CudaWarp<EXT> ex;
     ex.lane = lane;
-    if (wid == 0) kkt_warp_setup<EXT>(ex, c.variable_dt);
+    if (wid == 0) kkt_warp_setup<EXT>(ex, c0.variable_dt);
     __syncthreads();
     uint32_t parity = 0;
     unsigned long long cyc[MPCB200_NUM_PHASES] = {0, 0, 0, 0, 0}, cyc_total = 0, n_kkt = 0, n_sweeps = 0, n_inst = 0;
@@ -345,7 +363,7 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
     unsigned long long* sms = nullptr;
     // (PTX does not promise %smid < the SM count: a CTA without a word runs without gates)
     if (a.sm_sync) { const unsigned smid = sm_index(); if (smid < (unsigned)a.sm_words) sms = a.sm_sync + (size_t)smid * SMS_WORD_STRIDE; }
-    const int outer = c.outer_iterations > 0 ? c.outer_iterations : 1;
+    const int outer = c0.outer_iterations > 0 ? c0.outer_iterations : 1;
 // Phase clocks: EVERY thread keeps them (thread 0's are reported).  Not `if (tid == 0)`: a thread-0-only block directly in front of
 // warp-collective code (shuffles, votes) made the compiler split the paths of thread 0 and of lanes 1..31 through the KKT phase in
 // one build variant -- lanes 1..31 ran their shuffles on the converged fast path, thread 0 waited in the collective slow path for
@@ -387,9 +405,15 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
         // ---- inputs ----
         if (wid == 0)
         {
-            const bool ok = scatter_one<LINES>(L, W, a.in, src, lane, nullptr);
+            bool ok = scatter_one<LINES>(L, W, a.in, src, lane, nullptr);
             if (lane == 0)
             {
+                if (ROBOT && ok)   // the robot's configuration: its record, checked as the blocking setter checks it
+                {
+                    const double* rec = r.limits + (int64_t)src * MPCB200_LIMIT_WORDS;
+                    ok = robot_limits_valid(c0, rec);
+                    if (ok) apply_robot_limits(r.cfg[blockIdx.x], rec);
+                }
                 s_valid = ok; ASC(MPCB200_SC_VALID) = ok ? 1.0 : 0.0; if (!ok) mark_invalid(L, W);
                 if (MULTI && ok && rank > 0)   // a challenger: the straight line bumped by its rank, whatever the incumbent's plan
                 {
@@ -468,6 +492,18 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
         atomicAdd(a.counters + CNT_KKT_SWEEPS, n_sweeps);
         atomicAdd(a.counters + CNT_INST, n_inst);
     }
+}
+template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI>
+__global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve_fused_kernel(const __grid_constant__ Cfg c, const __grid_constant__ WsLayout L, const __grid_constant__ FusedArgs a)
+{
+    solve_fused<LINES, EXT, WARPS, MODEL, MULTI, false>(c, L, a, RobotArgs{nullptr, nullptr});
+}
+// the per-robot-limits form: the same solve, the phases read the configuration of the CTA's current robot (RobotArgs)
+template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI>
+__global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve_fused_robot_kernel(const __grid_constant__ Cfg c, const __grid_constant__ WsLayout L,
+                                                                                                   const __grid_constant__ FusedArgs a, const __grid_constant__ RobotArgs r)
+{
+    solve_fused<LINES, EXT, WARPS, MODEL, MULTI, true>(c, L, a, r);
 }
 
 // ---- kernel: multistart selection, one warp per robot: the winner among the K candidates (multistart_winner), its state into
@@ -604,6 +640,10 @@ struct mpcb200_handle
     int hist_B = 0;                  // batch size of the last batch solve whose iteration counts are in batch.iters (0: none)
     int *d_prev_iters = nullptr, *d_prev_status = nullptr, *d_order = nullptr;
     int* d_winner = nullptr;         // [max_batch] candidate index of each robot's winner (mpcb200_step_batch_multistart)
+    int robot_limits_n = 0;          // records of per-robot limits in d_limits (0: none, the solves run solve_fused_kernel)
+    double* d_limits = nullptr;      // [max_batch][MPCB200_LIMIT_WORDS]
+    Cfg* d_robot_cfg = nullptr;      // [robot_cfg_slots] configuration of each CTA of a solve_fused_robot_kernel launch
+    int robot_cfg_slots = 0;         // CTAs a solve launch can have: min(max_batch, 32 per SM)
     unsigned long long budget_ns = 0;          // max_cpu_time in ns (0: no budget)
     unsigned long long* d_origin = nullptr;    // start of the current solve launch (%globaltimer), see FusedArgs
     int sm_phase_sync = -1;          // MPCB200_OPT_SM_PHASE_SYNC: co-resident CTAs of the solve kernel enter the phases together
@@ -699,19 +739,31 @@ static cudaError_t allow_smem(K kernel) { return cudaFuncSetAttribute(kernel, cu
 // ---- the kernel variants: one table per kernel.  The variants compiled for one robot / footprint model (MODEL_UNI_POINT) exist
 //      without the line-obstacle paths only (LINES = false); a request for one with them gets the generic variant.  The fixed-dt
 //      quadratic-form key (MODEL_UNI_POINT_QF) exists for the unbordered KKT only (EXT = false). ----
-using FusedKernel = decltype(&solve_fused_kernel<false, false, SMALL_GROUP_WARPS, MODEL_GENERIC, false>);
-template <int WARPS, bool MULTI>
-static FusedKernel fused_shape_variant(bool lines, bool ext, int model)
+//      The per-robot-limits entries (solve_fused_robot_kernel) form a second table of the same variants.
+struct FusedEntry
 {
-    if (lines) return ext ? solve_fused_kernel<true, true, WARPS, MODEL_GENERIC, MULTI> : solve_fused_kernel<true, false, WARPS, MODEL_GENERIC, MULTI>;
-    if (model == MODEL_UNI_POINT_QF && !ext) return solve_fused_kernel<false, false, WARPS, MODEL_UNI_POINT_QF, MULTI>;
-    if (model == MODEL_UNI_POINT) return ext ? solve_fused_kernel<false, true, WARPS, MODEL_UNI_POINT, MULTI> : solve_fused_kernel<false, false, WARPS, MODEL_UNI_POINT, MULTI>;
-    return ext ? solve_fused_kernel<false, true, WARPS, MODEL_GENERIC, MULTI> : solve_fused_kernel<false, false, WARPS, MODEL_GENERIC, MULTI>;
+    template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI> static constexpr auto get() { return solve_fused_kernel<LINES, EXT, WARPS, MODEL, MULTI>; }
+};
+struct RobotEntry
+{
+    template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI> static constexpr auto get() { return solve_fused_robot_kernel<LINES, EXT, WARPS, MODEL, MULTI>; }
+};
+template <class E> using EntryKernel = decltype(E::template get<false, false, SMALL_GROUP_WARPS, MODEL_GENERIC, false>());
+using FusedKernel = EntryKernel<FusedEntry>;
+using RobotKernel = EntryKernel<RobotEntry>;
+template <class E, int WARPS, bool MULTI>
+static EntryKernel<E> fused_shape_variant(bool lines, bool ext, int model)
+{
+    if (lines) return ext ? E::template get<true, true, WARPS, MODEL_GENERIC, MULTI>() : E::template get<true, false, WARPS, MODEL_GENERIC, MULTI>();
+    if (model == MODEL_UNI_POINT_QF && !ext) return E::template get<false, false, WARPS, MODEL_UNI_POINT_QF, MULTI>();
+    if (model == MODEL_UNI_POINT) return ext ? E::template get<false, true, WARPS, MODEL_UNI_POINT, MULTI>() : E::template get<false, false, WARPS, MODEL_UNI_POINT, MULTI>();
+    return ext ? E::template get<false, true, WARPS, MODEL_GENERIC, MULTI>() : E::template get<false, false, WARPS, MODEL_GENERIC, MULTI>();
 }
-static FusedKernel fused_variant(bool lines, bool ext, bool small, int model, bool multi)
+template <class E = FusedEntry>
+static EntryKernel<E> fused_variant(bool lines, bool ext, bool small, int model, bool multi)
 {
-    if (multi) return small ? fused_shape_variant<SMALL_GROUP_WARPS, true>(lines, ext, model) : fused_shape_variant<MAX_GROUP_WARPS, true>(lines, ext, model);
-    return small ? fused_shape_variant<SMALL_GROUP_WARPS, false>(lines, ext, model) : fused_shape_variant<MAX_GROUP_WARPS, false>(lines, ext, model);
+    if (multi) return small ? fused_shape_variant<E, SMALL_GROUP_WARPS, true>(lines, ext, model) : fused_shape_variant<E, MAX_GROUP_WARPS, true>(lines, ext, model);
+    return small ? fused_shape_variant<E, SMALL_GROUP_WARPS, false>(lines, ext, model) : fused_shape_variant<E, MAX_GROUP_WARPS, false>(lines, ext, model);
 }
 using PhaseKernel = decltype(&phase_kernel<false, MODEL_GENERIC>);
 static PhaseKernel phase_variant(bool lines, int model)
@@ -837,6 +889,8 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
     }
     CKC(cudaMalloc(&h->d_nactive, 8)); CKC(cudaMalloc(&h->d_queue, 4)); CKC(cudaMalloc(&h->d_smsync, (size_t)h->num_sms * SMS_WORD_STRIDE * 8)); CKC(cudaMalloc(&h->d_prev_iters, B * 4)); CKC(cudaMalloc(&h->d_prev_status, B * 4)); CKC(cudaMalloc(&h->d_order, (B + 2) * 4));
     CKC(cudaMalloc(&h->d_origin, 8)); CKC(cudaMalloc(&h->d_winner, B * 4));
+    h->robot_cfg_slots = max_batch < 32 * h->num_sms ? max_batch : 32 * h->num_sms;
+    CKC(cudaMalloc(&h->d_limits, B * MPCB200_LIMIT_WORDS * 8)); CKC(cudaMalloc(&h->d_robot_cfg, (size_t)h->robot_cfg_slots * sizeof(Cfg)));
     CKC(cudaMalloc(&h->d_counters, CNT_BYTES)); CKC(cudaMemsetAsync(h->d_counters, 0, CNT_BYTES, h->stream));
     CKC(allow_smem(kkt_warp_kernel<false>)); CKC(allow_smem(kkt_warp_kernel<true>));
     for (const bool lines : {false, true})
@@ -845,7 +899,11 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
             CKC(allow_smem(phase_variant(lines, model)));
             for (const bool ext : {false, true})
                 for (const bool small : {false, true})
-                    for (const bool multi : {false, true}) CKC(allow_smem(fused_variant(lines, ext, small, model, multi)));
+                    for (const bool multi : {false, true})
+                    {
+                        CKC(allow_smem(fused_variant(lines, ext, small, model, multi)));
+                        CKC(allow_smem(fused_variant<RobotEntry>(lines, ext, small, model, multi)));
+                    }
         }
     CKC(cudaMallocHost(&h->h_nactive, 8));
     CKC(cudaEventCreateWithFlags(&h->poll_ev[0], cudaEventDisableTiming)); CKC(cudaEventCreateWithFlags(&h->poll_ev[1], cudaEventDisableTiming));
@@ -874,7 +932,7 @@ extern "C" void mpcb200_destroy(mpcb200_handle* h)
     io_release(h->batch);
     io_release(h->queue);
     void* ptrs[] = {h->ws, h->d_nactive, h->d_queue, h->d_flush, h->d_counters, h->d_smsync, h->d_prev_iters, h->d_prev_status, h->d_order,
-                    h->d_origin, h->d_winner, h->d_resample, h->d_cm, h->d_fz};
+                    h->d_origin, h->d_winner, h->d_resample, h->d_cm, h->d_fz, h->d_limits, h->d_robot_cfg};
     for (void* p : ptrs) if (p) cudaFree(p);
     if (h->h_nactive) cudaFreeHost(h->h_nactive);
     for (auto& e : h->ev) cudaEventDestroy(e);
@@ -1059,12 +1117,16 @@ static int launch_fused(mpcb200_handle* h, const IoBuffers& io, int total, int q
     const size_t smem = IMG_HEAD + (size_t)a.img_words * 8;
     if (smem > MAX_IMG_SMEM) return set_err(h, MPCB200_E_UNSUPPORTED, "the instance does not fit in shared memory");
     const int threads = group_threads(h), model = kernel_model(h, io);
-    const FusedKernel kernel = fused_variant(io.has_lines, kkt_is_ext(h->cfg), threads <= SMALL_GROUP_WARPS * 32, model, cand_stride > 0);
+    const bool ext = kkt_is_ext(h->cfg), small = threads <= SMALL_GROUP_WARPS * 32, robot = h->robot_limits_n > 0 && !queue_mode;
+    const FusedKernel kernel = robot ? nullptr : fused_variant(io.has_lines, ext, small, model, cand_stride > 0);
+    const RobotKernel robot_kernel = robot ? fused_variant<RobotEntry>(io.has_lines, ext, small, model, cand_stride > 0) : nullptr;
     int per_sm = 0;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
+    if (robot) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, robot_kernel, threads, smem));
+    else CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
     if (per_sm < 1) return set_err(h, MPCB200_E_UNSUPPORTED, "the solve kernel does not fit on an SM with this configuration");
     if (h->max_ctas_per_sm > 0 && per_sm > h->max_ctas_per_sm) per_sm = h->max_ctas_per_sm;
     const int grid = total < per_sm * h->num_sms ? total : per_sm * h->num_sms;
+    if (robot && grid > h->robot_cfg_slots) return set_err(h, MPCB200_E_UNSUPPORTED, "more CTAs than per-robot configuration slots");
     h->fused_grid = grid;
     CK(cudaMemsetAsync(h->d_queue, 0, 4, h->stream));
     if (!queue_mode && h->order_by_history && h->hist_B == total && total > h->num_sms)
@@ -1086,7 +1148,8 @@ static int launch_fused(mpcb200_handle* h, const IoBuffers& io, int total, int q
     // phase alignment pays when several CTAs share an SM (auto: from three CTAs per SM)
     if (h->sm_phase_sync > 0 || (h->sm_phase_sync < 0 && per_sm >= 3 && grid > h->num_sms)) { a.sm_sync = h->d_smsync; a.sm_words = h->num_sms; }
     if (a.sm_sync || a.place) CK(cudaMemsetAsync(h->d_smsync, 0, (size_t)h->num_sms * SMS_WORD_STRIDE * 8, h->stream));
-    kernel<<<grid, threads, smem, h->stream>>>(h->cfg, h->L, a);
+    if (robot) robot_kernel<<<grid, threads, smem, h->stream>>>(h->cfg, h->L, a, RobotArgs{h->d_limits, h->d_robot_cfg});
+    else kernel<<<grid, threads, smem, h->stream>>>(h->cfg, h->L, a);
     h->last_model = model;
     h->stats.launches_total += 1;
     CK(cudaGetLastError());
@@ -1167,6 +1230,19 @@ static int check_budget_mode(mpcb200_handle* h)
     return 0;
 }
 
+// With per-robot limits set, a solve of `robots` robots needs a record for each, and the persistent kernel (the phased mode has no
+// per-robot form).  Checked before anything is enqueued.
+static int check_robot_limits(mpcb200_handle* h, int robots)
+{
+    if (h->robot_limits_n == 0) return 0;
+    if (h->solve_mode == 1)
+        return set_err(h, MPCB200_E_UNSUPPORTED, "per-robot limits need the fused solve kernel (MPCB200_OPT_SOLVE_MODE 0)");
+    if (robots > h->robot_limits_n)
+        return set_err(h, MPCB200_E_INVALID, "per-robot limits: " + std::to_string(robots) + " robots, " + std::to_string(h->robot_limits_n) +
+                                             " records (mpcb200_set_robot_limits)");
+    return 0;
+}
+
 // The solve of a batch on the device arrays: one launch of the persistent kernel.  Without a host synchronise behind it (the
 // device-memory calls), its counters are folded on the device with the launch's own grid.
 static int launch_solve_async(mpcb200_handle* h, const IoBuffers& io, int total)
@@ -1233,6 +1309,7 @@ extern "C" int mpcb200_solve_stream(mpcb200_handle* h, int total, const double* 
 {
     if (!h) return MPCB200_E_INVALID;
     if (total < 1 || !x0 || !xf) return set_err(h, MPCB200_E_INVALID, "total >= 1, x0 and xf are required");
+    if (h->robot_limits_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "solve_stream with per-robot limits: queue entries are not robots");
     CK(cudaSetDevice(h->device));
     int rc;
     if ((rc = io_reserve(h, h->queue, (size_t)total, 0))) return rc;
@@ -1249,6 +1326,7 @@ extern "C" int mpcb200_step_batch(mpcb200_handle* h, int B, const double* x0, co
     int rc = check_batch(h, B);
     if (rc) return rc;
     if ((rc = check_budget_mode(h))) return rc;
+    if ((rc = check_robot_limits(h, B))) return rc;
     CK(cudaSetDevice(h->device));
     if ((rc = load_inputs(h, h->batch, B, x0, xf, u_prev, u_prev_dt, obst, vp, x_init, reinit))) return rc;
     // the phased mode works on the instance blocks; the fused kernel reads the compact arrays itself
@@ -1273,6 +1351,7 @@ extern "C" int mpcb200_step_batch_multistart(mpcb200_handle* h, int B, int K, do
         return set_err(h, MPCB200_E_UNSUPPORTED, "multistart: the challengers' bumped lines are solver-side preprocessing, off with reference_initial_guess");
     if (K > 1 && h->cfg.initial_guess_bumps > 31) return set_err(h, MPCB200_E_UNSUPPORTED, "multistart: initial_guess_bumps <= 31 with K > 1");
     if (h->solve_mode == 1) return set_err(h, MPCB200_E_UNSUPPORTED, "multistart needs the fused solve kernel (MPCB200_OPT_SOLVE_MODE 0)");
+    if ((rc = check_robot_limits(h, B))) return rc;
     CK(cudaSetDevice(h->device));
     if ((rc = load_inputs(h, h->batch, B, x0, xf, u_prev, u_prev_dt, obst, vp, x_init, reinit))) return rc;
     h->B = B;
@@ -1299,6 +1378,7 @@ extern "C" int mpcb200_solve_resident(mpcb200_handle* h, int cold, double* solve
 {
     if (!h || h->B < 1) return set_err(h, MPCB200_E_INVALID, "no resident inputs: call mpcb200_upload_inputs first");
     if (int rc = check_budget_mode(h)) return rc;
+    if (int rc = check_robot_limits(h, h->B)) return rc;
     CK(cudaSetDevice(h->device));
     return timed_launch(h, h->batch, h->B, 0, cold ? 1 : 0, solve_time_s);
 }
@@ -1355,6 +1435,42 @@ extern "C" int mpcb200_get_horizon(const mpcb200_handle* h, int* n, int* n_capac
     if (!h) return MPCB200_E_INVALID;
     if (n) *n = h->cfg.n;
     if (n_capacity) *n_capacity = h->n_cap;
+    return MPCB200_OK;
+}
+
+// ---- per-robot limits: records into d_limits; the solves launch solve_fused_robot_kernel while robot_limits_n > 0 ----
+extern "C" int mpcb200_set_robot_limits(mpcb200_handle* h, int n, const double* limits)
+{
+    if (!h) return MPCB200_E_INVALID;
+    if (n < 0 || n > h->max_batch) return set_err(h, MPCB200_E_INVALID, "set_robot_limits: n must be in [0, max_batch]");
+    if (n > 0 && !limits) return set_err(h, MPCB200_E_INVALID, "set_robot_limits: limits are required for n > 0");
+    for (int b = 0; b < n; ++b)
+        if (!robot_limits_valid(h->cfg, limits + (size_t)b * MPCB200_LIMIT_WORDS))
+            return set_err(h, MPCB200_E_INVALID, "set_robot_limits: record " + std::to_string(b) + " is not valid (NaN, u_ub <= u_lb, a bound "
+                                                 "finite where the configuration's is not or the reverse, or a clearance not in [0, inf))");
+    CK(cudaSetDevice(h->device));
+    if (n > 0)
+    {
+        CK(cudaMemcpyAsync(h->d_limits, limits, (size_t)n * MPCB200_LIMIT_WORDS * 8, cudaMemcpyHostToDevice, h->stream));
+        h->stats.h2d_bytes += (long long)n * MPCB200_LIMIT_WORDS * 8;
+        CK(cudaStreamSynchronize(h->stream));
+    }
+    h->robot_limits_n = n;
+    return MPCB200_OK;
+}
+
+extern "C" int mpcb200_set_robot_limits_async(mpcb200_handle* h, int n, const double* limits)
+{
+    if (!h) return MPCB200_E_INVALID;
+    if (n < 0 || n > h->max_batch) return set_err(h, MPCB200_E_INVALID, "set_robot_limits_async: n must be in [0, max_batch]");
+    if (n > 0 && !limits) return set_err(h, MPCB200_E_INVALID, "set_robot_limits_async: limits are required for n > 0");
+    CK(cudaSetDevice(h->device));
+    if (n > 0)
+    {
+        if (int rc = check_device_arrays(h, "set_robot_limits_async", {limits})) return rc;
+        CK(cudaMemcpyAsync(h->d_limits, limits, (size_t)n * MPCB200_LIMIT_WORDS * 8, cudaMemcpyDeviceToDevice, h->stream));
+    }
+    h->robot_limits_n = n;
     return MPCB200_OK;
 }
 
@@ -1453,6 +1569,7 @@ extern "C" int mpcb200_run_phase(mpcb200_handle* h, int phase, int B)
 {
     int rc = check_batch(h, B);
     if (rc) return rc;
+    if (h->robot_limits_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot limits (mpcb200_set_robot_limits)");
     CK(cudaSetDevice(h->device));
     if ((rc = launch_phase(h, phase, B, 0, 1, nullptr, true))) return rc;
     CK(cudaStreamSynchronize(h->stream));
@@ -1495,6 +1612,7 @@ extern "C" int mpcb200_time_phase(mpcb200_handle* h, int phase, int B, int reps,
 {
     int rc = check_batch(h, B);
     if (rc) return rc;
+    if (h->robot_limits_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot limits (mpcb200_set_robot_limits)");
     if (reps < 1) reps = 1;
     CK(cudaSetDevice(h->device));
     double total = 0.0;
@@ -1650,6 +1768,7 @@ extern "C" int mpcb200_step_batch_costmap(mpcb200_handle* h, int B, const double
     if (rc) return rc;
     if (max_per_instance < 1 || max_per_instance > MAX_OBST_LIST) return set_err(h, MPCB200_E_UNSUPPORTED, "step_batch_costmap: 1..2048 obstacles per instance");
     if ((rc = check_budget_mode(h))) return rc;
+    if ((rc = check_robot_limits(h, B))) return rc;
     CK(cudaSetDevice(h->device));
     IoBuffers& io = h->batch;
     // room for the lists in the batch's obstacle arrays
@@ -1742,6 +1861,7 @@ extern "C" int mpcb200_step_batch_async(mpcb200_handle* h, int B, const double* 
     int rc = check_batch(h, B);
     if (rc) return rc;
     if ((rc = check_async(h, flags, MPCB200_ASYNC_LINE_OBSTACLES))) return rc;
+    if ((rc = check_robot_limits(h, B))) return rc;
     CK(cudaSetDevice(h->device));
     if ((rc = check_device_arrays(h, "step_batch_async", {x0, xf, u_prev, obst ? obst->count : nullptr, obst ? obst->type : nullptr,
                                                           obst ? obst->params : nullptr, vp ? vp->count : nullptr, vp ? vp->poses : nullptr,
@@ -1763,6 +1883,7 @@ extern "C" int mpcb200_step_batch_costmap_async(mpcb200_handle* h, int B, const 
     if (rc) return rc;
     if (max_per_instance < 1 || max_per_instance > MAX_OBST_LIST) return set_err(h, MPCB200_E_UNSUPPORTED, "step_batch_costmap: 1..2048 obstacles per instance");
     if ((rc = check_async(h, 0u, 0u))) return rc;
+    if ((rc = check_robot_limits(h, B))) return rc;
     if (!maps) return set_err(h, MPCB200_E_INVALID, "costmap_obstacles: B >= 1, maps, poses and output arrays are required");
     CK(cudaSetDevice(h->device));
     if ((rc = check_device_arrays(h, "step_batch_costmap_async", {maps->cost, maps->origin, x0, xf, u_prev, vp ? vp->count : nullptr,
