@@ -288,6 +288,42 @@ int mpcb200_set_robot_limits(mpcb200_handle* h, int n, const double* limits);
 int mpcb200_set_robot_limits_async(mpcb200_handle* h, int n, const double* limits);
 
 /*
+ * Per-robot geometry: robots of different sizes and steering geometry in one handle and one solve launch (the reference's
+ * per-Controller footprint model, src/mpc_local_planner_ros.cpp:890-1028, and robot/simple_car/wheelbase,
+ * robot/kinematic_bicycle_vel_input/length_rear | length_front, src/controller.cpp:494-549).  A record is MPCB200_GEOMETRY_WORDS
+ * doubles:
+ *   [MPCB200_GEO_WHEELBASE]              wheelbase
+ *   [MPCB200_GEO_LENGTH_REAR]            length_rear          [MPCB200_GEO_LENGTH_FRONT]   length_front
+ *   [MPCB200_GEO_FOOTPRINT + i]          footprint_params[i]  (i = 0..3)
+ *   [MPCB200_GEO_N_POLY]                 n_poly, an integer held as a double
+ *   [MPCB200_GEO_POLY_XY + i]            poly_xy[i]           (i = 0 .. 2 * MPCB200_MAX_POLY - 1)
+ *   Values, not models.  robot_type and footprint_type stay properties of the handle, and so do the kernel variant and the kernel
+ *     key (mpcb200_kernel_model / _problem).  A record supplies the words the handle's two types read, and only those are used:
+ *     the wheelbase of either simple car, the two lengths of the kinematic bicycle; the radius of a circular footprint, the four
+ *     footprint words of two circles or a line, n_poly and the first n_poly vertices of a polygon.  Every other word is ignored
+ *     and may hold anything.  They are used wherever the configuration's are read: the dynamics and their derivatives, the
+ *     footprint distance of the obstacle rows, the association, the bumped-line scoring and the cold start's control seeding.  A
+ *     robot whose record changed between two calls warm-starts from its previous solution under the new values.
+ *   Validity (mpc_core.h robot_geometry_valid), of the words that are read: wheelbase finite and > 0; length_rear finite and > 0,
+ *     length_front finite and >= 0; radii finite and >= 0; offsets and line end points finite; n_poly integral in
+ *     [1, MPCB200_MAX_POLY] and its vertices finite.
+ *   A unicycle with a point footprint reads no geometry word: both setters return E_INVALID for n > 0 on such a handle.
+ *   Scope, the setters and the calls refused while records are set: as for the limits records above, word for word
+ *     (mpcb200_set_robot_geometry: host records, checked, E_INVALID and nothing changes when one is not valid;
+ *     mpcb200_set_robot_geometry_async: device records, checked per robot by the solve, an invalid one makes its robot
+ *     MPCB200_STATUS_INVALID_INPUT).  Limit and geometry records combine: a robot with both gets both.
+ */
+#define MPCB200_GEOMETRY_WORDS 40
+#define MPCB200_GEO_WHEELBASE 0
+#define MPCB200_GEO_LENGTH_REAR 1
+#define MPCB200_GEO_LENGTH_FRONT 2
+#define MPCB200_GEO_FOOTPRINT 3
+#define MPCB200_GEO_N_POLY 7
+#define MPCB200_GEO_POLY_XY 8
+int mpcb200_set_robot_geometry(mpcb200_handle* h, int n, const double* geometry);
+int mpcb200_set_robot_geometry_async(mpcb200_handle* h, int n, const double* geometry);
+
+/*
  * The same solves for a QUEUE of `total` instances (total may exceed max_batch by any factor): the handle's max_batch
  * workspaces form a pool of slots, and a slot whose instance has finished hands its result over and takes the next
  * instance of the queue while the other slots keep iterating (continuous batching).  The interior-point iterations of

@@ -143,6 +143,7 @@ class Controller
         }
         if (!setHorizon(_n_ref)) return false;
         if (_has_limits && !applyRobotLimits()) return false;
+        if (_has_geometry && !applyRobotGeometry()) return false;
         _ocp_seq = 0; _grid_empty = true; _ocp_successful = false;
         return true;
     }
@@ -167,6 +168,29 @@ class Controller
     {
         if (_h) mpcb200_set_robot_limits(_h, 0, nullptr);
         _has_limits = false;
+    }
+
+    // Runtime geometry of this robot (mpcb200_set_robot_geometry with one record, MPCB200_GEO_* words): the wheelbase or the
+    // bicycle's lengths and the footprint's values in place of the configuration's (a cart picked up, a tool extended).  The robot
+    // and footprint types stay the configuration's.  This is the footprint change of the reference without a reconfigure: the next
+    // step warm-starts under the new values.  They survive reset(), grid adaptation and a new configure(); false (and the previous
+    // geometry kept) when the record is not valid for the configuration (mpcb200.h).
+    bool setRobotGeometry(const double geometry[MPCB200_GEOMETRY_WORDS])
+    {
+        if (_h && mpcb200_set_robot_geometry(_h, 1, geometry) != MPCB200_OK)
+        {
+            std::fprintf(stderr, "Controller::setRobotGeometry(): %s\n", mpcb200_last_error(_h));
+            return false;
+        }
+        for (int i = 0; i < MPCB200_GEOMETRY_WORDS; ++i) _geometry[i] = geometry[i];
+        _has_geometry = true;
+        return true;
+    }
+    // back to the configuration's geometry
+    void clearRobotGeometry()
+    {
+        if (_h) mpcb200_set_robot_geometry(_h, 0, nullptr);
+        _has_geometry = false;
     }
 
     // StructuredOptimalControlProblem::setPreviousControlInput (called by the planner before step, src/mpc_local_planner_ros.cpp:384)
@@ -328,6 +352,12 @@ class Controller
         std::fprintf(stderr, "Controller: robot limits: %s\n", mpcb200_last_error(_h));
         return false;
     }
+    bool applyRobotGeometry()
+    {
+        if (mpcb200_set_robot_geometry(_h, 1, _geometry) == MPCB200_OK) return true;
+        std::fprintf(stderr, "Controller: robot geometry: %s\n", mpcb200_last_error(_h));
+        return false;
+    }
     static void fill(TimeSeries& ts, const std::vector<double>& v, int dim, int N, double dt)
     {
         ts.clear(); ts.dim = dim;
@@ -351,6 +381,8 @@ class Controller
     int _last_status = -1, _last_iters = 0;
     double _limits[MPCB200_LIMIT_WORDS] = {};
     bool _has_limits = false;   // setRobotLimits in effect
+    double _geometry[MPCB200_GEOMETRY_WORDS] = {};
+    bool _has_geometry = false; // setRobotGeometry in effect
 };
 
 }  // namespace mpcb200

@@ -42,6 +42,9 @@ ASYNC_LINE_OBSTACLES = 1
 # per-robot limits (mpcb200_set_robot_limits): words of a record
 LIMIT_WORDS = 9
 LIM_U_LB, LIM_U_UB, LIM_DU_LB, LIM_DU_UB, LIM_MIN_OBSTACLE_DIST = 0, 2, 4, 6, 8
+# per-robot geometry (mpcb200_set_robot_geometry): words of a record
+GEOMETRY_WORDS = 40
+GEO_WHEELBASE, GEO_LENGTH_REAR, GEO_LENGTH_FRONT, GEO_FOOTPRINT, GEO_N_POLY, GEO_POLY_XY = 0, 1, 2, 3, 7, 8
 SOLVE_FUSED, SOLVE_PHASED = 0, 1
 NUM_PHASES = 5
 K_H, K_G, K_A, K_B, K_E, K_C, K_HB, K_D = 0, 15, 20, 23, 29, 32, 34, 39
@@ -213,6 +216,7 @@ EXPORTS = [
     "mpcb200_step_batch_async", "mpcb200_step_batch_costmap_async", "mpcb200_check_feasible_async",
     "mpcb200_step_batch_multistart",
     "mpcb200_set_robot_limits", "mpcb200_set_robot_limits_async",
+    "mpcb200_set_robot_geometry", "mpcb200_set_robot_geometry_async",
 ]
 
 
@@ -238,6 +242,8 @@ def load_library(path=None):
                                                   C.POINTER(ViaPoints), dp, ucp, dp, dp, dp, ip, dp, ip, ip, dp]
     lib.mpcb200_set_robot_limits.argtypes = [vp, C.c_int, dp]
     lib.mpcb200_set_robot_limits_async.argtypes = [vp, C.c_int, vp]
+    lib.mpcb200_set_robot_geometry.argtypes = [vp, C.c_int, dp]
+    lib.mpcb200_set_robot_geometry_async.argtypes = [vp, C.c_int, vp]
     lib.mpcb200_solve_stream.argtypes = [vp, C.c_int, dp, dp, dp, C.c_double, C.POINTER(Obstacles), C.POINTER(ViaPoints),
                                          dp, dp, dp, ip, dp, ip, dp]
     lib.mpcb200_reset.argtypes = [vp, ucp, C.c_int]
@@ -463,6 +469,29 @@ class BatchSolver:
             return
         p = _tensor_ptr(t, "limits", torch.float64, self.device, (None, LIMIT_WORDS))
         self._check(self.lib.mpcb200_set_robot_limits_async(self.h, int(t.shape[0]), p), "mpcb200_set_robot_limits_async")
+
+    def set_robot_geometry(self, a):
+        """Per-robot geometry (mpcb200_set_robot_geometry): a = [n, GEOMETRY_WORDS] (wheelbase, length_rear, length_front,
+        footprint_params[4], n_poly, poly_xy[32] per robot) replaces the values the handle's robot and footprint types read for
+        robots 0..n-1 of every later solve; the other words are ignored.  None clears."""
+        if a is None:
+            self._check(self.lib.mpcb200_set_robot_geometry(self.h, 0, None), "mpcb200_set_robot_geometry")
+            return
+        a = np.ascontiguousarray(a, dtype=np.float64)
+        if a.ndim != 2 or a.shape[1] != GEOMETRY_WORDS:
+            raise ValueError(f"geometry must have shape [n, {GEOMETRY_WORDS}], got {a.shape}")
+        self._check(self.lib.mpcb200_set_robot_geometry(self.h, a.shape[0], _dp(a)), "mpcb200_set_robot_geometry")
+
+    def set_robot_geometry_async(self, t):
+        """set_robot_geometry() from a torch CUDA tensor float64 [n, GEOMETRY_WORDS] (mpcb200_set_robot_geometry_async): copied on
+        the handle's stream, which must be torch's current stream; the solve checks each robot's record (an invalid one makes its
+        robot STATUS_INVALID_INPUT).  None clears."""
+        torch = self._async_prologue()
+        if t is None:
+            self._check(self.lib.mpcb200_set_robot_geometry_async(self.h, 0, None), "mpcb200_set_robot_geometry_async")
+            return
+        p = _tensor_ptr(t, "geometry", torch.float64, self.device, (None, GEOMETRY_WORDS))
+        self._check(self.lib.mpcb200_set_robot_geometry_async(self.h, int(t.shape[0]), p), "mpcb200_set_robot_geometry_async")
 
     def upload(self, x0, xf, u_prev=None, u_prev_dt=0.0, obstacles=None, viapoints=None, x_init=None):
         B, x0, xf, u_prev, o, v, xi, keep = self._prep_inputs(x0, xf, u_prev, obstacles, viapoints, x_init)

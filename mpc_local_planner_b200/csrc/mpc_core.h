@@ -152,6 +152,77 @@ HD inline void apply_robot_limits(Cfg& c, const double* r)
     c.min_obstacle_dist = r[MPCB200_LIM_MIN_OBSTACLE_DIST];
 }
 
+// ---- per-robot geometry (mpcb200_set_robot_geometry): a record of MPCB200_GEOMETRY_WORDS doubles ----
+// robot_type and footprint_type stay the handle's; a record supplies the values those two types read and nothing else, so the
+// check and the patch look at exactly those words (the others may hold anything, NaN included).  The blocking setter checks every
+// record with this on the host, the solve kernel checks the record of each robot with it in the instance's prologue.
+HD inline bool geo_finite(double v) { return v >= -1.7976931348623157e308 && v <= 1.7976931348623157e308; }
+HD inline bool robot_geometry_valid(const Cfg& c, const double* r)
+{
+    switch (c.robot_type)
+    {
+        case MPCB200_ROBOT_SIMPLE_CAR:
+        case MPCB200_ROBOT_SIMPLE_CAR_FRONT:
+            if (!(geo_finite(r[MPCB200_GEO_WHEELBASE]) && r[MPCB200_GEO_WHEELBASE] > 0.0)) return false;
+            break;
+        case MPCB200_ROBOT_KIN_BICYCLE:
+            if (!(geo_finite(r[MPCB200_GEO_LENGTH_REAR]) && r[MPCB200_GEO_LENGTH_REAR] > 0.0)) return false;
+            if (!(geo_finite(r[MPCB200_GEO_LENGTH_FRONT]) && r[MPCB200_GEO_LENGTH_FRONT] >= 0.0)) return false;
+            break;
+        default: break;
+    }
+    const double* f = r + MPCB200_GEO_FOOTPRINT;
+    switch (c.footprint_type)
+    {
+        case MPCB200_FOOTPRINT_CIRCULAR: return geo_finite(f[0]) && f[0] >= 0.0;
+        case MPCB200_FOOTPRINT_TWO_CIRCLES:   // front offset, front radius, rear offset, rear radius
+            return geo_finite(f[0]) && geo_finite(f[2]) && geo_finite(f[1]) && f[1] >= 0.0 && geo_finite(f[3]) && f[3] >= 0.0;
+        case MPCB200_FOOTPRINT_LINE: return geo_finite(f[0]) && geo_finite(f[1]) && geo_finite(f[2]) && geo_finite(f[3]);
+        case MPCB200_FOOTPRINT_POLYGON:
+        {
+            const double np = r[MPCB200_GEO_N_POLY];
+            if (!(np >= 1.0 && np <= (double)MPCB200_MAX_POLY) || np != floor(np)) return false;
+            for (int i = 0; i < 2 * (int)np; ++i)
+                if (!geo_finite(r[MPCB200_GEO_POLY_XY + i])) return false;
+            return true;
+        }
+        default: return true;
+    }
+}
+// the configuration of a robot: the record's values of the fields its robot and footprint types read, every other field untouched
+// (polygon vertices past n_poly included: nothing reads them)
+HD inline void apply_robot_geometry(Cfg& c, const double* r)
+{
+    switch (c.robot_type)
+    {
+        case MPCB200_ROBOT_SIMPLE_CAR:
+        case MPCB200_ROBOT_SIMPLE_CAR_FRONT: c.wheelbase = r[MPCB200_GEO_WHEELBASE]; break;
+        case MPCB200_ROBOT_KIN_BICYCLE:
+            c.length_rear = r[MPCB200_GEO_LENGTH_REAR];
+            c.length_front = r[MPCB200_GEO_LENGTH_FRONT];
+            break;
+        default: break;
+    }
+    switch (c.footprint_type)
+    {
+        case MPCB200_FOOTPRINT_CIRCULAR: c.footprint_params[0] = r[MPCB200_GEO_FOOTPRINT]; break;
+        case MPCB200_FOOTPRINT_TWO_CIRCLES:
+        case MPCB200_FOOTPRINT_LINE:
+            for (int i = 0; i < 4; ++i) c.footprint_params[i] = r[MPCB200_GEO_FOOTPRINT + i];
+            break;
+        case MPCB200_FOOTPRINT_POLYGON:
+            c.n_poly = (int)r[MPCB200_GEO_N_POLY];
+            for (int i = 0; i < 2 * c.n_poly; ++i) c.poly_xy[i] = r[MPCB200_GEO_POLY_XY + i];
+            break;
+        default: break;
+    }
+}
+// a handle whose robot and footprint types read no geometry word (a unicycle with a point footprint): nothing to vary
+HD inline bool reads_geometry(const Cfg& c)
+{
+    return c.robot_type != MPCB200_ROBOT_UNICYCLE || c.footprint_type != MPCB200_FOOTPRINT_POINT;
+}
+
 // ---- model / problem key of a kernel variant ----
 // MODEL_GENERIC reads the robot and footprint model from the configuration at run time.  MODEL_UNI_POINT is compiled for the
 // unicycle with a point footprint (the BASELINE configurations 2, 4 and 5): the tests of the two fields fold at compile time and the

@@ -320,8 +320,10 @@ struct RobotArgs
 // ROBOT: the per-robot-limits form.  Either only changes the prologue of an instance (MULTI: its inputs, its bump rank; ROBOT: the
 // configuration the phases read), and each is an instantiation of its own, so that the solve kernels of the other calls keep their
 // registers and local memory.
-template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI, bool ROBOT>
-__device__ __forceinline__ void solve_fused(const Cfg& c0, const WsLayout& L, const FusedArgs& a, const RobotArgs& r)
+// FLEET (with ROBOT): the per-robot-geometry form -- the limits records are optional (r.limits may be null), and the geometry
+// record of each robot (mpcb200_set_robot_geometry, `geo`) is applied to the CTA's configuration after them.
+template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI, bool ROBOT, bool FLEET = false>
+__device__ __forceinline__ void solve_fused(const Cfg& c0, const WsLayout& L, const FusedArgs& a, const RobotArgs& r, const double* geo = nullptr)
 {
     const Cfg& c = ROBOT ? r.cfg[blockIdx.x] : c0;
     extern __shared__ __align__(128) unsigned char dyn_smem[];
@@ -410,9 +412,29 @@ __device__ __forceinline__ void solve_fused(const Cfg& c0, const WsLayout& L, co
             {
                 if (ROBOT && ok)   // the robot's configuration: its record, checked as the blocking setter checks it
                 {
-                    const double* rec = r.limits + (int64_t)src * MPCB200_LIMIT_WORDS;
-                    ok = robot_limits_valid(c0, rec);
-                    if (ok) apply_robot_limits(r.cfg[blockIdx.x], rec);
+                    if constexpr (FLEET)
+                    {
+                        // every field a phase reads is rewritten here for each instance: nothing of the CTA's previous robot is left
+                        Cfg& rc = r.cfg[blockIdx.x];
+                        if (r.limits)
+                        {
+                            const double* rec = r.limits + (int64_t)src * MPCB200_LIMIT_WORDS;
+                            ok = robot_limits_valid(c0, rec);
+                            if (ok) apply_robot_limits(rc, rec);
+                        }
+                        if (ok)
+                        {
+                            const double* g = geo + (int64_t)src * MPCB200_GEOMETRY_WORDS;
+                            ok = robot_geometry_valid(c0, g);
+                            if (ok) apply_robot_geometry(rc, g);
+                        }
+                    }
+                    else
+                    {
+                        const double* rec = r.limits + (int64_t)src * MPCB200_LIMIT_WORDS;
+                        ok = robot_limits_valid(c0, rec);
+                        if (ok) apply_robot_limits(r.cfg[blockIdx.x], rec);
+                    }
                 }
                 s_valid = ok; ASC(MPCB200_SC_VALID) = ok ? 1.0 : 0.0; if (!ok) mark_invalid(L, W);
                 if (MULTI && ok && rank > 0)   // a challenger: the straight line bumped by its rank, whatever the incumbent's plan
@@ -504,6 +526,15 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
                                                                                                    const __grid_constant__ FusedArgs a, const __grid_constant__ RobotArgs r)
 {
     solve_fused<LINES, EXT, WARPS, MODEL, MULTI, true>(c, L, a, r);
+}
+// the per-robot-geometry form (built for MODEL_GENERIC only: a handle with geometry records never has the unicycle / point key):
+// the same solve, the CTA's configuration patched with its current robot's limits record, if any, and geometry record
+template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI>
+__global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve_fused_fleet_kernel(const __grid_constant__ Cfg c, const __grid_constant__ WsLayout L,
+                                                                                                   const __grid_constant__ FusedArgs a, const __grid_constant__ RobotArgs r,
+                                                                                                   const double* geometry)
+{
+    solve_fused<LINES, EXT, WARPS, MODEL, MULTI, true, true>(c, L, a, r, geometry);
 }
 
 // ---- kernel: multistart selection, one warp per robot: the winner among the K candidates (multistart_winner), its state into
@@ -642,7 +673,9 @@ struct mpcb200_handle
     int* d_winner = nullptr;         // [max_batch] candidate index of each robot's winner (mpcb200_step_batch_multistart)
     int robot_limits_n = 0;          // records of per-robot limits in d_limits (0: none, the solves run solve_fused_kernel)
     double* d_limits = nullptr;      // [max_batch][MPCB200_LIMIT_WORDS]
-    Cfg* d_robot_cfg = nullptr;      // [robot_cfg_slots] configuration of each CTA of a solve_fused_robot_kernel launch
+    int robot_geometry_n = 0;        // records of per-robot geometry in d_geometry (0: none; > 0: the solves run solve_fused_fleet_kernel)
+    double* d_geometry = nullptr;    // [max_batch][MPCB200_GEOMETRY_WORDS]
+    Cfg* d_robot_cfg = nullptr;      // [robot_cfg_slots] configuration of each CTA of a solve_fused_robot_kernel / _fleet_kernel launch
     int robot_cfg_slots = 0;         // CTAs a solve launch can have: min(max_batch, 32 per SM)
     unsigned long long budget_ns = 0;          // max_cpu_time in ns (0: no budget)
     unsigned long long* d_origin = nullptr;    // start of the current solve launch (%globaltimer), see FusedArgs
@@ -739,7 +772,8 @@ static cudaError_t allow_smem(K kernel) { return cudaFuncSetAttribute(kernel, cu
 // ---- the kernel variants: one table per kernel.  The variants compiled for one robot / footprint model (MODEL_UNI_POINT) exist
 //      without the line-obstacle paths only (LINES = false); a request for one with them gets the generic variant.  The fixed-dt
 //      quadratic-form key (MODEL_UNI_POINT_QF) exists for the unbordered KKT only (EXT = false). ----
-//      The per-robot-limits entries (solve_fused_robot_kernel) form a second table of the same variants.
+//      The per-robot-limits entries (solve_fused_robot_kernel) form a second table of the same variants, the per-robot-geometry
+//      entries (solve_fused_fleet_kernel) a third one of the MODEL_GENERIC variants.
 struct FusedEntry
 {
     template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI> static constexpr auto get() { return solve_fused_kernel<LINES, EXT, WARPS, MODEL, MULTI>; }
@@ -748,9 +782,15 @@ struct RobotEntry
 {
     template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI> static constexpr auto get() { return solve_fused_robot_kernel<LINES, EXT, WARPS, MODEL, MULTI>; }
 };
+// the per-robot-geometry entries (solve_fused_fleet_kernel) exist for MODEL_GENERIC only: every key maps to it
+struct FleetEntry
+{
+    template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI> static constexpr auto get() { return solve_fused_fleet_kernel<LINES, EXT, WARPS, MODEL_GENERIC, MULTI>; }
+};
 template <class E> using EntryKernel = decltype(E::template get<false, false, SMALL_GROUP_WARPS, MODEL_GENERIC, false>());
 using FusedKernel = EntryKernel<FusedEntry>;
 using RobotKernel = EntryKernel<RobotEntry>;
+using FleetKernel = EntryKernel<FleetEntry>;
 template <class E, int WARPS, bool MULTI>
 static EntryKernel<E> fused_shape_variant(bool lines, bool ext, int model)
 {
@@ -891,6 +931,7 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
     CKC(cudaMalloc(&h->d_origin, 8)); CKC(cudaMalloc(&h->d_winner, B * 4));
     h->robot_cfg_slots = max_batch < 32 * h->num_sms ? max_batch : 32 * h->num_sms;
     CKC(cudaMalloc(&h->d_limits, B * MPCB200_LIMIT_WORDS * 8)); CKC(cudaMalloc(&h->d_robot_cfg, (size_t)h->robot_cfg_slots * sizeof(Cfg)));
+    CKC(cudaMalloc(&h->d_geometry, B * MPCB200_GEOMETRY_WORDS * 8));
     CKC(cudaMalloc(&h->d_counters, CNT_BYTES)); CKC(cudaMemsetAsync(h->d_counters, 0, CNT_BYTES, h->stream));
     CKC(allow_smem(kkt_warp_kernel<false>)); CKC(allow_smem(kkt_warp_kernel<true>));
     for (const bool lines : {false, true})
@@ -903,6 +944,7 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
                     {
                         CKC(allow_smem(fused_variant(lines, ext, small, model, multi)));
                         CKC(allow_smem(fused_variant<RobotEntry>(lines, ext, small, model, multi)));
+                        if (model == MODEL_GENERIC) CKC(allow_smem(fused_variant<FleetEntry>(lines, ext, small, model, multi)));
                     }
         }
     CKC(cudaMallocHost(&h->h_nactive, 8));
@@ -932,7 +974,8 @@ extern "C" void mpcb200_destroy(mpcb200_handle* h)
     io_release(h->batch);
     io_release(h->queue);
     void* ptrs[] = {h->ws, h->d_nactive, h->d_queue, h->d_flush, h->d_counters, h->d_smsync, h->d_prev_iters, h->d_prev_status, h->d_order,
-                    h->d_origin, h->d_winner, h->d_resample, h->d_cm, h->d_fz, h->d_limits, h->d_robot_cfg};
+                    h->d_origin, h->d_winner, h->d_resample, h->d_cm, h->d_fz, h->d_limits, h->d_robot_cfg,
+                    h->d_geometry};
     for (void* p : ptrs) if (p) cudaFree(p);
     if (h->h_nactive) cudaFreeHost(h->h_nactive);
     for (auto& e : h->ev) cudaEventDestroy(e);
@@ -1118,15 +1161,20 @@ static int launch_fused(mpcb200_handle* h, const IoBuffers& io, int total, int q
     if (smem > MAX_IMG_SMEM) return set_err(h, MPCB200_E_UNSUPPORTED, "the instance does not fit in shared memory");
     const int threads = group_threads(h), model = kernel_model(h, io);
     const bool ext = kkt_is_ext(h->cfg), small = threads <= SMALL_GROUP_WARPS * 32, robot = h->robot_limits_n > 0 && !queue_mode;
-    const FusedKernel kernel = robot ? nullptr : fused_variant(io.has_lines, ext, small, model, cand_stride > 0);
-    const RobotKernel robot_kernel = robot ? fused_variant<RobotEntry>(io.has_lines, ext, small, model, cand_stride > 0) : nullptr;
+    // geometry records: the fleet entry, which applies the limits records too when there are any
+    const bool fleet = h->robot_geometry_n > 0 && !queue_mode;
+    if (fleet && model != MODEL_GENERIC) return set_err(h, MPCB200_E_UNSUPPORTED, "per-robot geometry needs the generic kernel variant");
+    const FusedKernel kernel = robot || fleet ? nullptr : fused_variant(io.has_lines, ext, small, model, cand_stride > 0);
+    const RobotKernel robot_kernel = robot && !fleet ? fused_variant<RobotEntry>(io.has_lines, ext, small, model, cand_stride > 0) : nullptr;
+    const FleetKernel fleet_kernel = fleet ? fused_variant<FleetEntry>(io.has_lines, ext, small, model, cand_stride > 0) : nullptr;
     int per_sm = 0;
-    if (robot) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, robot_kernel, threads, smem));
+    if (fleet) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fleet_kernel, threads, smem));
+    else if (robot) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, robot_kernel, threads, smem));
     else CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
     if (per_sm < 1) return set_err(h, MPCB200_E_UNSUPPORTED, "the solve kernel does not fit on an SM with this configuration");
     if (h->max_ctas_per_sm > 0 && per_sm > h->max_ctas_per_sm) per_sm = h->max_ctas_per_sm;
     const int grid = total < per_sm * h->num_sms ? total : per_sm * h->num_sms;
-    if (robot && grid > h->robot_cfg_slots) return set_err(h, MPCB200_E_UNSUPPORTED, "more CTAs than per-robot configuration slots");
+    if ((robot || fleet) && grid > h->robot_cfg_slots) return set_err(h, MPCB200_E_UNSUPPORTED, "more CTAs than per-robot configuration slots");
     h->fused_grid = grid;
     CK(cudaMemsetAsync(h->d_queue, 0, 4, h->stream));
     if (!queue_mode && h->order_by_history && h->hist_B == total && total > h->num_sms)
@@ -1148,7 +1196,9 @@ static int launch_fused(mpcb200_handle* h, const IoBuffers& io, int total, int q
     // phase alignment pays when several CTAs share an SM (auto: from three CTAs per SM)
     if (h->sm_phase_sync > 0 || (h->sm_phase_sync < 0 && per_sm >= 3 && grid > h->num_sms)) { a.sm_sync = h->d_smsync; a.sm_words = h->num_sms; }
     if (a.sm_sync || a.place) CK(cudaMemsetAsync(h->d_smsync, 0, (size_t)h->num_sms * SMS_WORD_STRIDE * 8, h->stream));
-    if (robot) robot_kernel<<<grid, threads, smem, h->stream>>>(h->cfg, h->L, a, RobotArgs{h->d_limits, h->d_robot_cfg});
+    if (fleet)
+        fleet_kernel<<<grid, threads, smem, h->stream>>>(h->cfg, h->L, a, RobotArgs{robot ? h->d_limits : nullptr, h->d_robot_cfg}, h->d_geometry);
+    else if (robot) robot_kernel<<<grid, threads, smem, h->stream>>>(h->cfg, h->L, a, RobotArgs{h->d_limits, h->d_robot_cfg});
     else kernel<<<grid, threads, smem, h->stream>>>(h->cfg, h->L, a);
     h->last_model = model;
     h->stats.launches_total += 1;
@@ -1230,16 +1280,20 @@ static int check_budget_mode(mpcb200_handle* h)
     return 0;
 }
 
-// With per-robot limits set, a solve of `robots` robots needs a record for each, and the persistent kernel (the phased mode has no
-// per-robot form).  Checked before anything is enqueued.
+// With per-robot limits or geometry set, a solve of `robots` robots needs a record of each kind set for each, and the persistent
+// kernel (the phased mode has no per-robot form).  Checked before anything is enqueued.
 static int check_robot_limits(mpcb200_handle* h, int robots)
 {
-    if (h->robot_limits_n == 0) return 0;
+    if (h->robot_limits_n == 0 && h->robot_geometry_n == 0) return 0;
     if (h->solve_mode == 1)
-        return set_err(h, MPCB200_E_UNSUPPORTED, "per-robot limits need the fused solve kernel (MPCB200_OPT_SOLVE_MODE 0)");
-    if (robots > h->robot_limits_n)
+        return set_err(h, MPCB200_E_UNSUPPORTED, std::string(h->robot_limits_n > 0 ? "per-robot limits need" : "per-robot geometry needs") +
+                                                 " the fused solve kernel (MPCB200_OPT_SOLVE_MODE 0)");
+    if (h->robot_limits_n > 0 && robots > h->robot_limits_n)
         return set_err(h, MPCB200_E_INVALID, "per-robot limits: " + std::to_string(robots) + " robots, " + std::to_string(h->robot_limits_n) +
                                              " records (mpcb200_set_robot_limits)");
+    if (h->robot_geometry_n > 0 && robots > h->robot_geometry_n)
+        return set_err(h, MPCB200_E_INVALID, "per-robot geometry: " + std::to_string(robots) + " robots, " + std::to_string(h->robot_geometry_n) +
+                                             " records (mpcb200_set_robot_geometry)");
     return 0;
 }
 
@@ -1310,6 +1364,7 @@ extern "C" int mpcb200_solve_stream(mpcb200_handle* h, int total, const double* 
     if (!h) return MPCB200_E_INVALID;
     if (total < 1 || !x0 || !xf) return set_err(h, MPCB200_E_INVALID, "total >= 1, x0 and xf are required");
     if (h->robot_limits_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "solve_stream with per-robot limits: queue entries are not robots");
+    if (h->robot_geometry_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "solve_stream with per-robot geometry: queue entries are not robots");
     CK(cudaSetDevice(h->device));
     int rc;
     if ((rc = io_reserve(h, h->queue, (size_t)total, 0))) return rc;
@@ -1474,6 +1529,47 @@ extern "C" int mpcb200_set_robot_limits_async(mpcb200_handle* h, int n, const do
     return MPCB200_OK;
 }
 
+// ---- per-robot geometry: records into d_geometry; the solves launch solve_fused_fleet_kernel while robot_geometry_n > 0 ----
+extern "C" int mpcb200_set_robot_geometry(mpcb200_handle* h, int n, const double* geometry)
+{
+    if (!h) return MPCB200_E_INVALID;
+    if (n < 0 || n > h->max_batch) return set_err(h, MPCB200_E_INVALID, "set_robot_geometry: n must be in [0, max_batch]");
+    if (n > 0 && !geometry) return set_err(h, MPCB200_E_INVALID, "set_robot_geometry: geometry is required for n > 0");
+    if (n > 0 && !reads_geometry(h->cfg))
+        return set_err(h, MPCB200_E_INVALID, "set_robot_geometry: a unicycle with a point footprint has no geometry to vary");
+    for (int b = 0; b < n; ++b)
+        if (!robot_geometry_valid(h->cfg, geometry + (size_t)b * MPCB200_GEOMETRY_WORDS))
+            return set_err(h, MPCB200_E_INVALID, "set_robot_geometry: record " + std::to_string(b) + " is not valid (a wheelbase or length_rear "
+                                                 "not finite and > 0, a length_front or radius not finite and >= 0, an offset, line end or vertex "
+                                                 "not finite, or n_poly not an integer in [1, 16])");
+    CK(cudaSetDevice(h->device));
+    if (n > 0)
+    {
+        CK(cudaMemcpyAsync(h->d_geometry, geometry, (size_t)n * MPCB200_GEOMETRY_WORDS * 8, cudaMemcpyHostToDevice, h->stream));
+        h->stats.h2d_bytes += (long long)n * MPCB200_GEOMETRY_WORDS * 8;
+        CK(cudaStreamSynchronize(h->stream));
+    }
+    h->robot_geometry_n = n;
+    return MPCB200_OK;
+}
+
+extern "C" int mpcb200_set_robot_geometry_async(mpcb200_handle* h, int n, const double* geometry)
+{
+    if (!h) return MPCB200_E_INVALID;
+    if (n < 0 || n > h->max_batch) return set_err(h, MPCB200_E_INVALID, "set_robot_geometry_async: n must be in [0, max_batch]");
+    if (n > 0 && !geometry) return set_err(h, MPCB200_E_INVALID, "set_robot_geometry_async: geometry is required for n > 0");
+    if (n > 0 && !reads_geometry(h->cfg))
+        return set_err(h, MPCB200_E_INVALID, "set_robot_geometry_async: a unicycle with a point footprint has no geometry to vary");
+    CK(cudaSetDevice(h->device));
+    if (n > 0)
+    {
+        if (int rc = check_device_arrays(h, "set_robot_geometry_async", {geometry})) return rc;
+        CK(cudaMemcpyAsync(h->d_geometry, geometry, (size_t)n * MPCB200_GEOMETRY_WORDS * 8, cudaMemcpyDeviceToDevice, h->stream));
+    }
+    h->robot_geometry_n = n;
+    return MPCB200_OK;
+}
+
 // ---- kernel-level access ------------------------------------------------------------------------------------
 static int field_info(const mpcb200_handle* h, int field, int* off, int* cnt)
 {
@@ -1570,6 +1666,7 @@ extern "C" int mpcb200_run_phase(mpcb200_handle* h, int phase, int B)
     int rc = check_batch(h, B);
     if (rc) return rc;
     if (h->robot_limits_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot limits (mpcb200_set_robot_limits)");
+    if (h->robot_geometry_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot geometry (mpcb200_set_robot_geometry)");
     CK(cudaSetDevice(h->device));
     if ((rc = launch_phase(h, phase, B, 0, 1, nullptr, true))) return rc;
     CK(cudaStreamSynchronize(h->stream));
@@ -1613,6 +1710,7 @@ extern "C" int mpcb200_time_phase(mpcb200_handle* h, int phase, int B, int reps,
     int rc = check_batch(h, B);
     if (rc) return rc;
     if (h->robot_limits_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot limits (mpcb200_set_robot_limits)");
+    if (h->robot_geometry_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot geometry (mpcb200_set_robot_geometry)");
     if (reps < 1) reps = 1;
     CK(cudaSetDevice(h->device));
     double total = 0.0;
