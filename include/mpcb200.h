@@ -324,6 +324,39 @@ int mpcb200_set_robot_geometry(mpcb200_handle* h, int n, const double* geometry)
 int mpcb200_set_robot_geometry_async(mpcb200_handle* h, int n, const double* geometry);
 
 /*
+ * Per-robot weights: robots with different objective weights in one handle and one solve launch (the reference's per-Controller
+ * planning/objective/quadratic_form/state_weights | control_weights, src/controller.cpp:561-586; planning/terminal_cost/quadratic/
+ * final_state_weights, :652-661; planning/objective/minimum_time_via_points/position_weight | orientation_weight, :630-634).  A record
+ * is MPCB200_WEIGHT_WORDS doubles, the matrices row-major as in the configuration:
+ *   [MPCB200_WGT_Q + i]                  Q[i]                 (i = 0..8)
+ *   [MPCB200_WGT_R + i]                  R[i]                 (i = 0..3)
+ *   [MPCB200_WGT_QF + i]                 Qf[i]                (i = 0..8)
+ *   [MPCB200_WGT_VP_POSITION]            vp_position_weight   [MPCB200_WGT_VP_ORIENTATION]   vp_orientation_weight
+ *   Values, not terms.  The objective, terminal_cost, the via-point mode and hybrid_cost_minimum_time stay properties of the handle,
+ *     and so do the kernel variant and the kernel key (mpcb200_kernel_model / _problem).  A record supplies the words the handle's
+ *     objective reads, and only those are used: Q and R for the quadratic form (plain or hybrid), Qf with a terminal cost (any
+ *     objective), the two via-point weights with via-points.  Every other word is ignored and may hold anything.  A robot whose
+ *     record changed between two calls warm-starts from its previous solution under the new values.
+ *   Validity (mpc_core.h robot_weights_valid): every word that is read is finite, and the hybrid minimum-time term is on for the
+ *     record exactly when it is on for the handle (on a hybrid handle Q stays all zero and R not all zero; on a handle whose hybrid
+ *     flag fell back to the plain quadratic form a record cannot switch it on).  No definiteness test, as at mpcb200_create.
+ *   A handle that reads no weight (a minimum-time objective without terminal cost) refuses records: both setters return E_INVALID
+ *     for n > 0.
+ *   Scope, the setters and the calls refused while records are set: as for the limits records above, word for word
+ *     (mpcb200_set_robot_weights: host records, checked, E_INVALID and nothing changes when one is not valid;
+ *     mpcb200_set_robot_weights_async: device records, checked per robot by the solve, an invalid one makes its robot
+ *     MPCB200_STATUS_INVALID_INPUT).  Weights combine with limit and geometry records: a robot with all three gets all three.
+ */
+#define MPCB200_WEIGHT_WORDS 24
+#define MPCB200_WGT_Q 0
+#define MPCB200_WGT_R 9
+#define MPCB200_WGT_QF 13
+#define MPCB200_WGT_VP_POSITION 22
+#define MPCB200_WGT_VP_ORIENTATION 23
+int mpcb200_set_robot_weights(mpcb200_handle* h, int n, const double* weights);
+int mpcb200_set_robot_weights_async(mpcb200_handle* h, int n, const double* weights);
+
+/*
  * The same solves for a QUEUE of `total` instances (total may exceed max_batch by any factor): the handle's max_batch
  * workspaces form a pool of slots, and a slot whose instance has finished hands its result over and takes the next
  * instance of the queue while the other slots keep iterating (continuous batching).  The interior-point iterations of

@@ -144,6 +144,7 @@ class Controller
         if (!setHorizon(_n_ref)) return false;
         if (_has_limits && !applyRobotLimits()) return false;
         if (_has_geometry && !applyRobotGeometry()) return false;
+        if (_has_weights && !applyRobotWeights()) return false;
         _ocp_seq = 0; _grid_empty = true; _ocp_successful = false;
         return true;
     }
@@ -191,6 +192,29 @@ class Controller
     {
         if (_h) mpcb200_set_robot_geometry(_h, 0, nullptr);
         _has_geometry = false;
+    }
+
+    // Runtime objective weights of this robot (mpcb200_set_robot_weights with one record, MPCB200_WGT_* words): Q, R, Qf and the
+    // via-point weights in place of the configuration's (a heavier heading or terminal weight near the goal, smoother control with
+    // a load).  The objective and its terms stay the configuration's.  The next step warm-starts under the new values.  They
+    // survive reset(), grid adaptation and a new configure(); false (and the previous weights kept) when the record is not valid
+    // for the configuration (mpcb200.h).
+    bool setRobotWeights(const double weights[MPCB200_WEIGHT_WORDS])
+    {
+        if (_h && mpcb200_set_robot_weights(_h, 1, weights) != MPCB200_OK)
+        {
+            std::fprintf(stderr, "Controller::setRobotWeights(): %s\n", mpcb200_last_error(_h));
+            return false;
+        }
+        for (int i = 0; i < MPCB200_WEIGHT_WORDS; ++i) _weights[i] = weights[i];
+        _has_weights = true;
+        return true;
+    }
+    // back to the configuration's weights
+    void clearRobotWeights()
+    {
+        if (_h) mpcb200_set_robot_weights(_h, 0, nullptr);
+        _has_weights = false;
     }
 
     // StructuredOptimalControlProblem::setPreviousControlInput (called by the planner before step, src/mpc_local_planner_ros.cpp:384)
@@ -358,6 +382,12 @@ class Controller
         std::fprintf(stderr, "Controller: robot geometry: %s\n", mpcb200_last_error(_h));
         return false;
     }
+    bool applyRobotWeights()
+    {
+        if (mpcb200_set_robot_weights(_h, 1, _weights) == MPCB200_OK) return true;
+        std::fprintf(stderr, "Controller: robot weights: %s\n", mpcb200_last_error(_h));
+        return false;
+    }
     static void fill(TimeSeries& ts, const std::vector<double>& v, int dim, int N, double dt)
     {
         ts.clear(); ts.dim = dim;
@@ -383,6 +413,8 @@ class Controller
     bool _has_limits = false;   // setRobotLimits in effect
     double _geometry[MPCB200_GEOMETRY_WORDS] = {};
     bool _has_geometry = false; // setRobotGeometry in effect
+    double _weights[MPCB200_WEIGHT_WORDS] = {};
+    bool _has_weights = false;  // setRobotWeights in effect
 };
 
 }  // namespace mpcb200

@@ -45,6 +45,9 @@ LIM_U_LB, LIM_U_UB, LIM_DU_LB, LIM_DU_UB, LIM_MIN_OBSTACLE_DIST = 0, 2, 4, 6, 8
 # per-robot geometry (mpcb200_set_robot_geometry): words of a record
 GEOMETRY_WORDS = 40
 GEO_WHEELBASE, GEO_LENGTH_REAR, GEO_LENGTH_FRONT, GEO_FOOTPRINT, GEO_N_POLY, GEO_POLY_XY = 0, 1, 2, 3, 7, 8
+# per-robot weights (mpcb200_set_robot_weights): words of a record
+WEIGHT_WORDS = 24
+WGT_Q, WGT_R, WGT_QF, WGT_VP_POSITION, WGT_VP_ORIENTATION = 0, 9, 13, 22, 23
 SOLVE_FUSED, SOLVE_PHASED = 0, 1
 NUM_PHASES = 5
 K_H, K_G, K_A, K_B, K_E, K_C, K_HB, K_D = 0, 15, 20, 23, 29, 32, 34, 39
@@ -217,6 +220,7 @@ EXPORTS = [
     "mpcb200_step_batch_multistart",
     "mpcb200_set_robot_limits", "mpcb200_set_robot_limits_async",
     "mpcb200_set_robot_geometry", "mpcb200_set_robot_geometry_async",
+    "mpcb200_set_robot_weights", "mpcb200_set_robot_weights_async",
 ]
 
 
@@ -244,6 +248,8 @@ def load_library(path=None):
     lib.mpcb200_set_robot_limits_async.argtypes = [vp, C.c_int, vp]
     lib.mpcb200_set_robot_geometry.argtypes = [vp, C.c_int, dp]
     lib.mpcb200_set_robot_geometry_async.argtypes = [vp, C.c_int, vp]
+    lib.mpcb200_set_robot_weights.argtypes = [vp, C.c_int, dp]
+    lib.mpcb200_set_robot_weights_async.argtypes = [vp, C.c_int, vp]
     lib.mpcb200_solve_stream.argtypes = [vp, C.c_int, dp, dp, dp, C.c_double, C.POINTER(Obstacles), C.POINTER(ViaPoints),
                                          dp, dp, dp, ip, dp, ip, dp]
     lib.mpcb200_reset.argtypes = [vp, ucp, C.c_int]
@@ -492,6 +498,29 @@ class BatchSolver:
             return
         p = _tensor_ptr(t, "geometry", torch.float64, self.device, (None, GEOMETRY_WORDS))
         self._check(self.lib.mpcb200_set_robot_geometry_async(self.h, int(t.shape[0]), p), "mpcb200_set_robot_geometry_async")
+
+    def set_robot_weights(self, a):
+        """Per-robot weights (mpcb200_set_robot_weights): a = [n, WEIGHT_WORDS] (Q[9], R[4], Qf[9] row-major, vp_position_weight,
+        vp_orientation_weight per robot) replaces the weights the handle's objective reads for robots 0..n-1 of every later solve;
+        the other words are ignored.  None clears."""
+        if a is None:
+            self._check(self.lib.mpcb200_set_robot_weights(self.h, 0, None), "mpcb200_set_robot_weights")
+            return
+        a = np.ascontiguousarray(a, dtype=np.float64)
+        if a.ndim != 2 or a.shape[1] != WEIGHT_WORDS:
+            raise ValueError(f"weights must have shape [n, {WEIGHT_WORDS}], got {a.shape}")
+        self._check(self.lib.mpcb200_set_robot_weights(self.h, a.shape[0], _dp(a)), "mpcb200_set_robot_weights")
+
+    def set_robot_weights_async(self, t):
+        """set_robot_weights() from a torch CUDA tensor float64 [n, WEIGHT_WORDS] (mpcb200_set_robot_weights_async): copied on the
+        handle's stream, which must be torch's current stream; the solve checks each robot's record (an invalid one makes its robot
+        STATUS_INVALID_INPUT).  None clears."""
+        torch = self._async_prologue()
+        if t is None:
+            self._check(self.lib.mpcb200_set_robot_weights_async(self.h, 0, None), "mpcb200_set_robot_weights_async")
+            return
+        p = _tensor_ptr(t, "weights", torch.float64, self.device, (None, WEIGHT_WORDS))
+        self._check(self.lib.mpcb200_set_robot_weights_async(self.h, int(t.shape[0]), p), "mpcb200_set_robot_weights_async")
 
     def upload(self, x0, xf, u_prev=None, u_prev_dt=0.0, obstacles=None, viapoints=None, x_init=None):
         B, x0, xf, u_prev, o, v, xi, keep = self._prep_inputs(x0, xf, u_prev, obstacles, viapoints, x_init)

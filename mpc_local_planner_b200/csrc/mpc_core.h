@@ -223,6 +223,47 @@ HD inline bool reads_geometry(const Cfg& c)
     return c.robot_type != MPCB200_ROBOT_UNICYCLE || c.footprint_type != MPCB200_FOOTPRINT_POINT;
 }
 
+// ---- per-robot weights (mpcb200_set_robot_weights): a record of MPCB200_WEIGHT_WORDS doubles ----
+// The objective, the terminal-cost switch and the via-point mode stay the handle's; a record supplies the weights the handle's
+// objective reads (Q and R for the quadratic form, Qf with a terminal cost, the two via-point weights with via-points) and nothing
+// else, so the check and the patch look at exactly those words (the others may hold anything, NaN included).  The hybrid
+// minimum-time term is on for a quadratic form of zero Q and non-zero R (has_hybrid_mintime): a record keeps it as the handle has
+// it, so has_mintime, the kernel variant and key, and the variable_dt rule of mpcb200_create hold for every robot.  No definiteness
+// test: mpcb200_create makes none either.  The blocking setter checks every record with this on the host, the solve kernel checks
+// the record of each robot with it in the instance's prologue.
+HD inline bool reads_weights(const Cfg& c) { return has_quadratic(c) || has_terminal_cost(c) || has_viapoints(c); }
+HD inline bool robot_weights_valid(const Cfg& c, const double* r)
+{
+    if (has_quadratic(c))
+    {
+        bool qz = true, rz = true;
+        for (int i = 0; i < 9; ++i) { if (!geo_finite(r[MPCB200_WGT_Q + i])) return false; qz = qz && r[MPCB200_WGT_Q + i] == 0.0; }
+        for (int i = 0; i < 4; ++i) { if (!geo_finite(r[MPCB200_WGT_R + i])) return false; rz = rz && r[MPCB200_WGT_R + i] == 0.0; }
+        if ((c.hybrid_cost_minimum_time && qz && !rz) != has_hybrid_mintime(c)) return false;
+    }
+    if (has_terminal_cost(c))
+        for (int i = 0; i < 9; ++i)
+            if (!geo_finite(r[MPCB200_WGT_QF + i])) return false;
+    if (has_viapoints(c) && !(geo_finite(r[MPCB200_WGT_VP_POSITION]) && geo_finite(r[MPCB200_WGT_VP_ORIENTATION]))) return false;
+    return true;
+}
+// the configuration of a robot: the record's values of the weights its objective reads, every other field untouched
+HD inline void apply_robot_weights(Cfg& c, const double* r)
+{
+    if (has_quadratic(c))
+    {
+        for (int i = 0; i < 9; ++i) c.Q[i] = r[MPCB200_WGT_Q + i];
+        for (int i = 0; i < 4; ++i) c.R[i] = r[MPCB200_WGT_R + i];
+    }
+    if (has_terminal_cost(c))
+        for (int i = 0; i < 9; ++i) c.Qf[i] = r[MPCB200_WGT_QF + i];
+    if (has_viapoints(c))
+    {
+        c.vp_position_weight = r[MPCB200_WGT_VP_POSITION];
+        c.vp_orientation_weight = r[MPCB200_WGT_VP_ORIENTATION];
+    }
+}
+
 // ---- model / problem key of a kernel variant ----
 // MODEL_GENERIC reads the robot and footprint model from the configuration at run time.  MODEL_UNI_POINT is compiled for the
 // unicycle with a point footprint (the BASELINE configurations 2, 4 and 5): the tests of the two fields fold at compile time and the

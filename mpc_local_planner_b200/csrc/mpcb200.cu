@@ -27,7 +27,9 @@
 #include <vector>
 
 #include "mpc_device.cuh"
+#ifndef MPCB200_WEIGHTS_UNIT
 #include "mpc_costmap.cuh"
+#endif
 #include "mpc_gate.h"
 #include "mpc_place.h"
 
@@ -47,6 +49,9 @@
 // (fold_counters_kernel): cycle words as cycles per CTA of their own launch, the other words as counts
 #define CNT_BYTES (CNT_WORDS * 8 * 2)
 
+// mpcb200_weights.cu compiles this file with MPCB200_WEIGHTS_UNIT defined: the device code the solve kernel is made of and the
+// kernel-variant tables, without the other kernels and the host side, for the per-robot-weights entries it instantiates.
+#ifndef MPCB200_WEIGHTS_UNIT
 // ---- kernel: inputs of a batch into the instance blocks (phased path; the fused kernel scatters into shared memory itself) ----
 __global__ void scatter_inputs_kernel(WsLayout L, double* ws, int B, InputPtrs in)
 {
@@ -56,6 +61,7 @@ __global__ void scatter_inputs_kernel(WsLayout L, double* ws, int B, InputPtrs i
     const bool ok = scatter_one<true>(L, W, in, warp, lane, W + L.oXINIT);   // (the phased mode serves the blocking calls only)
     if (lane == 0) ASC(MPCB200_SC_VALID) = ok ? 1.0 : 0.0;
 }
+#endif
 
 // stage [0, words) of an instance block in shared memory (one bulk-async copy) / write [0, words) back
 __device__ __forceinline__ void stage_in(double* W, const double* Gp, int words, uint32_t bar, uint32_t parity, int tid)
@@ -252,6 +258,7 @@ __device__ __forceinline__ int history_key(const int* prev_iters, const int* pre
     const int k = prev_status[i] == MPCB200_STATUS_MAX_TIME ? max_iter : prev_iters[i];
     return k < 0 ? 0 : (k > 1023 ? 1023 : k);
 }
+#ifndef MPCB200_WEIGHTS_UNIT
 __global__ void __launch_bounds__(1024) order_by_history_kernel(const int* __restrict__ prev_iters, const int* __restrict__ prev_status, int max_iter,
                                                                 int B, int* __restrict__ order, int* place, int slots, double rho,
                                                                 int max_heavy, int* queue)
@@ -296,6 +303,7 @@ __global__ void __launch_bounds__(1024) order_by_history_kernel(const int* __res
             if (history_key(prev_iters, prev_status, max_iter, i) == key) order[pos++] = i;
     }
 }
+#endif
 
 // CTA shapes of the solve kernel.  The launch bound sets the register budget of a thread (255 in both shapes), so it follows
 // the shape a launch uses: horizons up to 64 grid points run 1-2 warps, and their shared-memory image (about 55 KB at N = 50)
@@ -322,8 +330,11 @@ struct RobotArgs
 // registers and local memory.
 // FLEET (with ROBOT): the per-robot-geometry form -- the limits records are optional (r.limits may be null), and the geometry
 // record of each robot (mpcb200_set_robot_geometry, `geo`) is applied to the CTA's configuration after them.
-template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI, bool ROBOT, bool FLEET = false>
-__device__ __forceinline__ void solve_fused(const Cfg& c0, const WsLayout& L, const FusedArgs& a, const RobotArgs& r, const double* geo = nullptr)
+// WEIGHTS (with ROBOT): the per-robot-weights form -- the limits and geometry records are optional (r.limits, geo may be null; geometry
+// only in the MODEL_GENERIC instantiations), and the weights record of each robot (mpcb200_set_robot_weights, `wgt`) is applied last.
+template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI, bool ROBOT, bool FLEET = false, bool WEIGHTS = false>
+__device__ __forceinline__ void solve_fused(const Cfg& c0, const WsLayout& L, const FusedArgs& a, const RobotArgs& r, const double* geo = nullptr,
+                                            const double* wgt = nullptr)
 {
     const Cfg& c = ROBOT ? r.cfg[blockIdx.x] : c0;
     extern __shared__ __align__(128) unsigned char dyn_smem[];
@@ -427,6 +438,30 @@ __device__ __forceinline__ void solve_fused(const Cfg& c0, const WsLayout& L, co
                             const double* g = geo + (int64_t)src * MPCB200_GEOMETRY_WORDS;
                             ok = robot_geometry_valid(c0, g);
                             if (ok) apply_robot_geometry(rc, g);
+                        }
+                    }
+                    else if constexpr (WEIGHTS)
+                    {
+                        // as FLEET: the limits, the geometry and the weights record each rewrite every field they touch, per instance
+                        Cfg& rc = r.cfg[blockIdx.x];
+                        if (r.limits)
+                        {
+                            const double* rec = r.limits + (int64_t)src * MPCB200_LIMIT_WORDS;
+                            ok = robot_limits_valid(c0, rec);
+                            if (ok) apply_robot_limits(rc, rec);
+                        }
+                        if constexpr (MODEL == MODEL_GENERIC)
+                            if (ok && geo)
+                            {
+                                const double* g = geo + (int64_t)src * MPCB200_GEOMETRY_WORDS;
+                                ok = robot_geometry_valid(c0, g);
+                                if (ok) apply_robot_geometry(rc, g);
+                            }
+                        if (ok)
+                        {
+                            const double* w = wgt + (int64_t)src * MPCB200_WEIGHT_WORDS;
+                            ok = robot_weights_valid(c0, w);
+                            if (ok) apply_robot_weights(rc, w);
                         }
                     }
                     else
@@ -536,7 +571,17 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
 {
     solve_fused<LINES, EXT, WARPS, MODEL, MULTI, true, true>(c, L, a, r, geometry);
 }
+// the per-robot-weights form (every key: weights are values of the quadratic-form terms the fixed-dt key keeps): the same solve, the
+// CTA's configuration patched with its current robot's limits record, if any, geometry record, if any, and weights record
+template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI>
+__global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve_fused_weights_kernel(const __grid_constant__ Cfg c, const __grid_constant__ WsLayout L,
+                                                                                                     const __grid_constant__ FusedArgs a, const __grid_constant__ RobotArgs r,
+                                                                                                     const double* geometry, const double* weights)
+{
+    solve_fused<LINES, EXT, WARPS, MODEL, MULTI, true, false, true>(c, L, a, r, geometry, weights);
+}
 
+#ifndef MPCB200_WEIGHTS_UNIT
 // ---- kernel: multistart selection, one warp per robot: the winner among the K candidates (multistart_winner), its state into
 //      slot b (and the resident obstacles' list indices of a long list), its results into output row b ----
 __global__ void multistart_select_kernel(WsLayout L, double* ws, int B, int K, double hysteresis, int long_list, OutputPtrs o, int* winner)
@@ -675,7 +720,9 @@ struct mpcb200_handle
     double* d_limits = nullptr;      // [max_batch][MPCB200_LIMIT_WORDS]
     int robot_geometry_n = 0;        // records of per-robot geometry in d_geometry (0: none; > 0: the solves run solve_fused_fleet_kernel)
     double* d_geometry = nullptr;    // [max_batch][MPCB200_GEOMETRY_WORDS]
-    Cfg* d_robot_cfg = nullptr;      // [robot_cfg_slots] configuration of each CTA of a solve_fused_robot_kernel / _fleet_kernel launch
+    int robot_weights_n = 0;         // records of per-robot weights in d_weights (0: none; > 0: the solves run solve_fused_weights_kernel)
+    double* d_weights = nullptr;     // [max_batch][MPCB200_WEIGHT_WORDS]
+    Cfg* d_robot_cfg = nullptr;      // [robot_cfg_slots] configuration of each CTA of a solve_fused_robot / _fleet / _weights_kernel launch
     int robot_cfg_slots = 0;         // CTAs a solve launch can have: min(max_batch, 32 per SM)
     unsigned long long budget_ns = 0;          // max_cpu_time in ns (0: no budget)
     unsigned long long* d_origin = nullptr;    // start of the current solve launch (%globaltimer), see FusedArgs
@@ -768,12 +815,14 @@ static int validate_config(const mpcb200_config* c, std::string& why)
 
 template <class K>
 static cudaError_t allow_smem(K kernel) { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_IMG_SMEM); }
+#endif
 
 // ---- the kernel variants: one table per kernel.  The variants compiled for one robot / footprint model (MODEL_UNI_POINT) exist
 //      without the line-obstacle paths only (LINES = false); a request for one with them gets the generic variant.  The fixed-dt
 //      quadratic-form key (MODEL_UNI_POINT_QF) exists for the unbordered KKT only (EXT = false). ----
 //      The per-robot-limits entries (solve_fused_robot_kernel) form a second table of the same variants, the per-robot-geometry
-//      entries (solve_fused_fleet_kernel) a third one of the MODEL_GENERIC variants.
+//      entries (solve_fused_fleet_kernel) a third one of the MODEL_GENERIC variants, the per-robot-weights entries
+//      (solve_fused_weights_kernel) a fourth one of all the variants, compiled in mpcb200_weights.cu (weights_kernel_variant).
 struct FusedEntry
 {
     template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI> static constexpr auto get() { return solve_fused_kernel<LINES, EXT, WARPS, MODEL, MULTI>; }
@@ -788,9 +837,6 @@ struct FleetEntry
     template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI> static constexpr auto get() { return solve_fused_fleet_kernel<LINES, EXT, WARPS, MODEL_GENERIC, MULTI>; }
 };
 template <class E> using EntryKernel = decltype(E::template get<false, false, SMALL_GROUP_WARPS, MODEL_GENERIC, false>());
-using FusedKernel = EntryKernel<FusedEntry>;
-using RobotKernel = EntryKernel<RobotEntry>;
-using FleetKernel = EntryKernel<FleetEntry>;
 template <class E, int WARPS, bool MULTI>
 static EntryKernel<E> fused_shape_variant(bool lines, bool ext, int model)
 {
@@ -805,6 +851,13 @@ static EntryKernel<E> fused_variant(bool lines, bool ext, bool small, int model,
     if (multi) return small ? fused_shape_variant<E, SMALL_GROUP_WARPS, true>(lines, ext, model) : fused_shape_variant<E, MAX_GROUP_WARPS, true>(lines, ext, model);
     return small ? fused_shape_variant<E, SMALL_GROUP_WARPS, false>(lines, ext, model) : fused_shape_variant<E, MAX_GROUP_WARPS, false>(lines, ext, model);
 }
+// the per-robot-weights entry of a variant (mpcb200_weights.cu): its host function, for cudaFuncSetAttribute, the occupancy query
+// and cudaLaunchKernel
+const void* weights_kernel_variant(bool lines, bool ext, bool small, int model, bool multi);
+#ifndef MPCB200_WEIGHTS_UNIT
+using FusedKernel = EntryKernel<FusedEntry>;
+using RobotKernel = EntryKernel<RobotEntry>;
+using FleetKernel = EntryKernel<FleetEntry>;
 using PhaseKernel = decltype(&phase_kernel<false, MODEL_GENERIC>);
 static PhaseKernel phase_variant(bool lines, int model)
 {
@@ -932,6 +985,7 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
     h->robot_cfg_slots = max_batch < 32 * h->num_sms ? max_batch : 32 * h->num_sms;
     CKC(cudaMalloc(&h->d_limits, B * MPCB200_LIMIT_WORDS * 8)); CKC(cudaMalloc(&h->d_robot_cfg, (size_t)h->robot_cfg_slots * sizeof(Cfg)));
     CKC(cudaMalloc(&h->d_geometry, B * MPCB200_GEOMETRY_WORDS * 8));
+    CKC(cudaMalloc(&h->d_weights, B * MPCB200_WEIGHT_WORDS * 8));
     CKC(cudaMalloc(&h->d_counters, CNT_BYTES)); CKC(cudaMemsetAsync(h->d_counters, 0, CNT_BYTES, h->stream));
     CKC(allow_smem(kkt_warp_kernel<false>)); CKC(allow_smem(kkt_warp_kernel<true>));
     for (const bool lines : {false, true})
@@ -945,6 +999,7 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
                         CKC(allow_smem(fused_variant(lines, ext, small, model, multi)));
                         CKC(allow_smem(fused_variant<RobotEntry>(lines, ext, small, model, multi)));
                         if (model == MODEL_GENERIC) CKC(allow_smem(fused_variant<FleetEntry>(lines, ext, small, model, multi)));
+                        CKC(allow_smem(weights_kernel_variant(lines, ext, small, model, multi)));
                     }
         }
     CKC(cudaMallocHost(&h->h_nactive, 8));
@@ -975,7 +1030,7 @@ extern "C" void mpcb200_destroy(mpcb200_handle* h)
     io_release(h->queue);
     void* ptrs[] = {h->ws, h->d_nactive, h->d_queue, h->d_flush, h->d_counters, h->d_smsync, h->d_prev_iters, h->d_prev_status, h->d_order,
                     h->d_origin, h->d_winner, h->d_resample, h->d_cm, h->d_fz, h->d_limits, h->d_robot_cfg,
-                    h->d_geometry};
+                    h->d_geometry, h->d_weights};
     for (void* p : ptrs) if (p) cudaFree(p);
     if (h->h_nactive) cudaFreeHost(h->h_nactive);
     for (auto& e : h->ev) cudaEventDestroy(e);
@@ -1162,19 +1217,23 @@ static int launch_fused(mpcb200_handle* h, const IoBuffers& io, int total, int q
     const int threads = group_threads(h), model = kernel_model(h, io);
     const bool ext = kkt_is_ext(h->cfg), small = threads <= SMALL_GROUP_WARPS * 32, robot = h->robot_limits_n > 0 && !queue_mode;
     // geometry records: the fleet entry, which applies the limits records too when there are any
-    const bool fleet = h->robot_geometry_n > 0 && !queue_mode;
-    if (fleet && model != MODEL_GENERIC) return set_err(h, MPCB200_E_UNSUPPORTED, "per-robot geometry needs the generic kernel variant");
-    const FusedKernel kernel = robot || fleet ? nullptr : fused_variant(io.has_lines, ext, small, model, cand_stride > 0);
-    const RobotKernel robot_kernel = robot && !fleet ? fused_variant<RobotEntry>(io.has_lines, ext, small, model, cand_stride > 0) : nullptr;
+    const bool geometry = h->robot_geometry_n > 0 && !queue_mode;
+    if (geometry && model != MODEL_GENERIC) return set_err(h, MPCB200_E_UNSUPPORTED, "per-robot geometry needs the generic kernel variant");
+    // weights records: the weights entry, which applies the limits and geometry records too when there are any
+    const bool weights = h->robot_weights_n > 0 && !queue_mode, fleet = geometry && !weights;
+    const FusedKernel kernel = robot || geometry || weights ? nullptr : fused_variant(io.has_lines, ext, small, model, cand_stride > 0);
+    const RobotKernel robot_kernel = robot && !geometry && !weights ? fused_variant<RobotEntry>(io.has_lines, ext, small, model, cand_stride > 0) : nullptr;
     const FleetKernel fleet_kernel = fleet ? fused_variant<FleetEntry>(io.has_lines, ext, small, model, cand_stride > 0) : nullptr;
+    const void* weights_kernel = weights ? weights_kernel_variant(io.has_lines, ext, small, model, cand_stride > 0) : nullptr;
     int per_sm = 0;
-    if (fleet) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fleet_kernel, threads, smem));
+    if (weights) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, weights_kernel, threads, smem));
+    else if (fleet) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fleet_kernel, threads, smem));
     else if (robot) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, robot_kernel, threads, smem));
     else CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
     if (per_sm < 1) return set_err(h, MPCB200_E_UNSUPPORTED, "the solve kernel does not fit on an SM with this configuration");
     if (h->max_ctas_per_sm > 0 && per_sm > h->max_ctas_per_sm) per_sm = h->max_ctas_per_sm;
     const int grid = total < per_sm * h->num_sms ? total : per_sm * h->num_sms;
-    if ((robot || fleet) && grid > h->robot_cfg_slots) return set_err(h, MPCB200_E_UNSUPPORTED, "more CTAs than per-robot configuration slots");
+    if ((robot || geometry || weights) && grid > h->robot_cfg_slots) return set_err(h, MPCB200_E_UNSUPPORTED, "more CTAs than per-robot configuration slots");
     h->fused_grid = grid;
     CK(cudaMemsetAsync(h->d_queue, 0, 4, h->stream));
     if (!queue_mode && h->order_by_history && h->hist_B == total && total > h->num_sms)
@@ -1196,7 +1255,14 @@ static int launch_fused(mpcb200_handle* h, const IoBuffers& io, int total, int q
     // phase alignment pays when several CTAs share an SM (auto: from three CTAs per SM)
     if (h->sm_phase_sync > 0 || (h->sm_phase_sync < 0 && per_sm >= 3 && grid > h->num_sms)) { a.sm_sync = h->d_smsync; a.sm_words = h->num_sms; }
     if (a.sm_sync || a.place) CK(cudaMemsetAsync(h->d_smsync, 0, (size_t)h->num_sms * SMS_WORD_STRIDE * 8, h->stream));
-    if (fleet)
+    if (weights)
+    {
+        RobotArgs ra{robot ? h->d_limits : nullptr, h->d_robot_cfg};
+        const double *geo = geometry ? h->d_geometry : nullptr, *wgt = h->d_weights;
+        void* args[] = {&h->cfg, &h->L, &a, &ra, &geo, &wgt};
+        CK(cudaLaunchKernel(weights_kernel, dim3(grid), dim3(threads), args, smem, h->stream));
+    }
+    else if (fleet)
         fleet_kernel<<<grid, threads, smem, h->stream>>>(h->cfg, h->L, a, RobotArgs{robot ? h->d_limits : nullptr, h->d_robot_cfg}, h->d_geometry);
     else if (robot) robot_kernel<<<grid, threads, smem, h->stream>>>(h->cfg, h->L, a, RobotArgs{h->d_limits, h->d_robot_cfg});
     else kernel<<<grid, threads, smem, h->stream>>>(h->cfg, h->L, a);
@@ -1280,13 +1346,14 @@ static int check_budget_mode(mpcb200_handle* h)
     return 0;
 }
 
-// With per-robot limits or geometry set, a solve of `robots` robots needs a record of each kind set for each, and the persistent
-// kernel (the phased mode has no per-robot form).  Checked before anything is enqueued.
+// With per-robot limits, geometry or weights set, a solve of `robots` robots needs a record of each kind set for each, and the
+// persistent kernel (the phased mode has no per-robot form).  Checked before anything is enqueued.
 static int check_robot_limits(mpcb200_handle* h, int robots)
 {
-    if (h->robot_limits_n == 0 && h->robot_geometry_n == 0) return 0;
+    if (h->robot_limits_n == 0 && h->robot_geometry_n == 0 && h->robot_weights_n == 0) return 0;
     if (h->solve_mode == 1)
-        return set_err(h, MPCB200_E_UNSUPPORTED, std::string(h->robot_limits_n > 0 ? "per-robot limits need" : "per-robot geometry needs") +
+        return set_err(h, MPCB200_E_UNSUPPORTED, std::string(h->robot_limits_n > 0 ? "per-robot limits need" :
+                                                             h->robot_geometry_n > 0 ? "per-robot geometry needs" : "per-robot weights need") +
                                                  " the fused solve kernel (MPCB200_OPT_SOLVE_MODE 0)");
     if (h->robot_limits_n > 0 && robots > h->robot_limits_n)
         return set_err(h, MPCB200_E_INVALID, "per-robot limits: " + std::to_string(robots) + " robots, " + std::to_string(h->robot_limits_n) +
@@ -1294,6 +1361,9 @@ static int check_robot_limits(mpcb200_handle* h, int robots)
     if (h->robot_geometry_n > 0 && robots > h->robot_geometry_n)
         return set_err(h, MPCB200_E_INVALID, "per-robot geometry: " + std::to_string(robots) + " robots, " + std::to_string(h->robot_geometry_n) +
                                              " records (mpcb200_set_robot_geometry)");
+    if (h->robot_weights_n > 0 && robots > h->robot_weights_n)
+        return set_err(h, MPCB200_E_INVALID, "per-robot weights: " + std::to_string(robots) + " robots, " + std::to_string(h->robot_weights_n) +
+                                             " records (mpcb200_set_robot_weights)");
     return 0;
 }
 
@@ -1365,6 +1435,7 @@ extern "C" int mpcb200_solve_stream(mpcb200_handle* h, int total, const double* 
     if (total < 1 || !x0 || !xf) return set_err(h, MPCB200_E_INVALID, "total >= 1, x0 and xf are required");
     if (h->robot_limits_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "solve_stream with per-robot limits: queue entries are not robots");
     if (h->robot_geometry_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "solve_stream with per-robot geometry: queue entries are not robots");
+    if (h->robot_weights_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "solve_stream with per-robot weights: queue entries are not robots");
     CK(cudaSetDevice(h->device));
     int rc;
     if ((rc = io_reserve(h, h->queue, (size_t)total, 0))) return rc;
@@ -1570,6 +1641,46 @@ extern "C" int mpcb200_set_robot_geometry_async(mpcb200_handle* h, int n, const 
     return MPCB200_OK;
 }
 
+// ---- per-robot weights: records into d_weights; the solves launch solve_fused_weights_kernel while robot_weights_n > 0 ----
+extern "C" int mpcb200_set_robot_weights(mpcb200_handle* h, int n, const double* weights)
+{
+    if (!h) return MPCB200_E_INVALID;
+    if (n < 0 || n > h->max_batch) return set_err(h, MPCB200_E_INVALID, "set_robot_weights: n must be in [0, max_batch]");
+    if (n > 0 && !weights) return set_err(h, MPCB200_E_INVALID, "set_robot_weights: weights are required for n > 0");
+    if (n > 0 && !reads_weights(h->cfg))
+        return set_err(h, MPCB200_E_INVALID, "set_robot_weights: a minimum-time objective without terminal cost has no weights to vary");
+    for (int b = 0; b < n; ++b)
+        if (!robot_weights_valid(h->cfg, weights + (size_t)b * MPCB200_WEIGHT_WORDS))
+            return set_err(h, MPCB200_E_INVALID, "set_robot_weights: record " + std::to_string(b) + " is not valid (a weight that is read "
+                                                 "not finite, or Q and R switching the hybrid minimum-time term against the configuration)");
+    CK(cudaSetDevice(h->device));
+    if (n > 0)
+    {
+        CK(cudaMemcpyAsync(h->d_weights, weights, (size_t)n * MPCB200_WEIGHT_WORDS * 8, cudaMemcpyHostToDevice, h->stream));
+        h->stats.h2d_bytes += (long long)n * MPCB200_WEIGHT_WORDS * 8;
+        CK(cudaStreamSynchronize(h->stream));
+    }
+    h->robot_weights_n = n;
+    return MPCB200_OK;
+}
+
+extern "C" int mpcb200_set_robot_weights_async(mpcb200_handle* h, int n, const double* weights)
+{
+    if (!h) return MPCB200_E_INVALID;
+    if (n < 0 || n > h->max_batch) return set_err(h, MPCB200_E_INVALID, "set_robot_weights_async: n must be in [0, max_batch]");
+    if (n > 0 && !weights) return set_err(h, MPCB200_E_INVALID, "set_robot_weights_async: weights are required for n > 0");
+    if (n > 0 && !reads_weights(h->cfg))
+        return set_err(h, MPCB200_E_INVALID, "set_robot_weights_async: a minimum-time objective without terminal cost has no weights to vary");
+    CK(cudaSetDevice(h->device));
+    if (n > 0)
+    {
+        if (int rc = check_device_arrays(h, "set_robot_weights_async", {weights})) return rc;
+        CK(cudaMemcpyAsync(h->d_weights, weights, (size_t)n * MPCB200_WEIGHT_WORDS * 8, cudaMemcpyDeviceToDevice, h->stream));
+    }
+    h->robot_weights_n = n;
+    return MPCB200_OK;
+}
+
 // ---- kernel-level access ------------------------------------------------------------------------------------
 static int field_info(const mpcb200_handle* h, int field, int* off, int* cnt)
 {
@@ -1667,6 +1778,7 @@ extern "C" int mpcb200_run_phase(mpcb200_handle* h, int phase, int B)
     if (rc) return rc;
     if (h->robot_limits_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot limits (mpcb200_set_robot_limits)");
     if (h->robot_geometry_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot geometry (mpcb200_set_robot_geometry)");
+    if (h->robot_weights_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot weights (mpcb200_set_robot_weights)");
     CK(cudaSetDevice(h->device));
     if ((rc = launch_phase(h, phase, B, 0, 1, nullptr, true))) return rc;
     CK(cudaStreamSynchronize(h->stream));
@@ -1711,6 +1823,7 @@ extern "C" int mpcb200_time_phase(mpcb200_handle* h, int phase, int B, int reps,
     if (rc) return rc;
     if (h->robot_limits_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot limits (mpcb200_set_robot_limits)");
     if (h->robot_geometry_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot geometry (mpcb200_set_robot_geometry)");
+    if (h->robot_weights_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot weights (mpcb200_set_robot_weights)");
     if (reps < 1) reps = 1;
     CK(cudaSetDevice(h->device));
     double total = 0.0;
@@ -2201,3 +2314,4 @@ extern "C" int mpcb200_step_batch_multi(mpcb200_multi* m, int B, const double* x
     if (solve_time_s) { double mx = 0.0; for (double s_ : secs) mx = s_ > mx ? s_ : mx; *solve_time_s = mx; }
     return MPCB200_OK;
 }
+#endif  // MPCB200_WEIGHTS_UNIT

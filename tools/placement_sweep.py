@@ -1,7 +1,7 @@
 """Critical placement (MPCB200_OPT_CRITICAL_PLACEMENT) of one workload against its plan: the heavy-part threshold PLACE_RHO and the
 co-resident cap PLACE_COTENANTS are compile-time constants of the library, so each setting is a library of its own, e.g.
   nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -shared -ldl -DPLACE_RHO=1.5 \
-       -DPLACE_COTENANTS=1 -o /tmp/rho15c1.so mpc_local_planner_b200/csrc/mpcb200.cu
+       -DPLACE_COTENANTS=1 -o /tmp/rho15c1.so mpc_local_planner_b200/csrc/mpcb200.cu mpc_local_planner_b200/csrc/mpcb200_weights.cu
 Measured the way bench.py measures its headline: cold batch solves, L2 flushed before each, queue longest-first by the history of
 the warm-up solves.  Each round runs every library once with the placement on, and the in-tree library with it off, so the
 settings alternate; results must be identical across settings (checked).
