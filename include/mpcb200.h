@@ -297,8 +297,9 @@ int mpcb200_set_robot_limits_async(mpcb200_handle* h, int n, const double* limit
  *   [MPCB200_GEO_FOOTPRINT + i]          footprint_params[i]  (i = 0..3)
  *   [MPCB200_GEO_N_POLY]                 n_poly, an integer held as a double
  *   [MPCB200_GEO_POLY_XY + i]            poly_xy[i]           (i = 0 .. 2 * MPCB200_MAX_POLY - 1)
- *   Values, not models.  robot_type and footprint_type stay properties of the handle, and so do the kernel variant and the kernel
- *     key (mpcb200_kernel_model / _problem).  A record supplies the words the handle's two types read, and only those are used:
+ *   Values, not models.  robot_type and footprint_type stay properties of the handle unless model records are set (below), and so
+ *     do the kernel variant and the kernel key (mpcb200_kernel_model / _problem).  A record supplies the words the robot's two types
+ *     read (the handle's, or its model record's), and only those are used:
  *     the wheelbase of either simple car, the two lengths of the kinematic bicycle; the radius of a circular footprint, the four
  *     footprint words of two circles or a line, n_poly and the first n_poly vertices of a polygon.  Every other word is ignored
  *     and may hold anything.  They are used wherever the configuration's are read: the dynamics and their derivatives, the
@@ -307,7 +308,8 @@ int mpcb200_set_robot_limits_async(mpcb200_handle* h, int n, const double* limit
  *   Validity (mpc_core.h robot_geometry_valid), of the words that are read: wheelbase finite and > 0; length_rear finite and > 0,
  *     length_front finite and >= 0; radii finite and >= 0; offsets and line end points finite; n_poly integral in
  *     [1, MPCB200_MAX_POLY] and its vertices finite.
- *   A unicycle with a point footprint reads no geometry word: both setters return E_INVALID for n > 0 on such a handle.
+ *   A unicycle with a point footprint reads no geometry word: both setters return E_INVALID for n > 0 on such a handle while no
+ *     model records are set.  With model records set, each record is checked for its robot's types (mpcb200_set_robot_model).
  *   Scope, the setters and the calls refused while records are set: as for the limits records above, word for word
  *     (mpcb200_set_robot_geometry: host records, checked, E_INVALID and nothing changes when one is not valid;
  *     mpcb200_set_robot_geometry_async: device records, checked per robot by the solve, an invalid one makes its robot
@@ -333,7 +335,8 @@ int mpcb200_set_robot_geometry_async(mpcb200_handle* h, int n, const double* geo
  *   [MPCB200_WGT_QF + i]                 Qf[i]                (i = 0..8)
  *   [MPCB200_WGT_VP_POSITION]            vp_position_weight   [MPCB200_WGT_VP_ORIENTATION]   vp_orientation_weight
  *   Values, not terms.  The objective, terminal_cost, the via-point mode and hybrid_cost_minimum_time stay properties of the handle,
- *     and so do the kernel variant and the kernel key (mpcb200_kernel_model / _problem).  A record supplies the words the handle's
+ *     and so do the kernel variant and the kernel key (mpcb200_kernel_model / _problem) unless model records are set (below).  A
+ *     record supplies the words the handle's
  *     objective reads, and only those are used: Q and R for the quadratic form (plain or hybrid), Qf with a terminal cost (any
  *     objective), the two via-point weights with via-points.  Every other word is ignored and may hold anything.  A robot whose
  *     record changed between two calls warm-starts from its previous solution under the new values.
@@ -355,6 +358,44 @@ int mpcb200_set_robot_geometry_async(mpcb200_handle* h, int n, const double* geo
 #define MPCB200_WGT_VP_ORIENTATION 23
 int mpcb200_set_robot_weights(mpcb200_handle* h, int n, const double* weights);
 int mpcb200_set_robot_weights_async(mpcb200_handle* h, int n, const double* weights);
+
+/*
+ * Per-robot model: unicycles, car-likes and bicycles of any footprint type in one handle and one solve launch (the reference's
+ * per-Controller robot/type, src/controller.cpp:344-378, and footprint_model/type, src/mpc_local_planner_ros.cpp:890-1028).  A
+ * record is MPCB200_MODEL_WORDS doubles:
+ *   [MPCB200_MOD_ROBOT_TYPE]             robot_type           (MPCB200_ROBOT_*, an integer held as a double)
+ *   [MPCB200_MOD_FOOTPRINT_TYPE]         footprint_type       (MPCB200_FOOTPRINT_*, an integer held as a double)
+ *   Types, not rows.  A record changes the robot's robot_type and footprint_type and nothing else.  The row set (which bound and
+ *     control-rate rows exist, as for the limits records), the objective, the grid, the collocation and the kernel variant (line
+ *     obstacles, bordered KKT, CTA shape) stay properties of the handle.  A mixed fleet whose models need different limits combines
+ *     model records with limits records; a bound that some robots do not need is given a large finite value.
+ *   Geometry follows the robot's types.  The geometry a robot uses -- its geometry record when geometry records are set, else the
+ *     handle's configuration values -- must be valid for its types (mpc_core.h robot_model_valid: the rules of the geometry
+ *     records below, for the record's types).  Example: a polygon record on a handle whose n_poly is 0, with no geometry record, is
+ *     not valid.  The blocking setters (this one and mpcb200_set_robot_geometry) check each record against the records of the
+ *     other kind currently set by a blocking setter, and a change that would leave some robot with an invalid pair returns
+ *     E_INVALID and changes nothing -- clearing the model records while geometry records are set that the handle's own types
+ *     refuse included.  The async setters check nothing on the host; the solve checks each robot's pair in its prologue, and an
+ *     invalid pair makes only that robot MPCB200_STATUS_INVALID_INPUT.  A robot changing its footprint type sets the geometry
+ *     record first (one valid for the old and the new type, e.g. a radius and a polygon), then the model record.  An order every
+ *     handle accepts for a new fleet: model records of the handle's own types (valid with any geometry, and they let a unicycle /
+ *     point handle take geometry records), then the geometry records, then the robots' model records.
+ *   Kernel key.  While model records are set every solve runs the generic key: mpcb200_kernel_model / _problem report
+ *     MPCB200_MODEL_GENERIC / MPCB200_PROBLEM_GENERIC.  Once they are cleared the handle's own key comes back, so a unicycle /
+ *     point-footprint handle may host cars.  A robot whose model changed between two calls warm-starts from its previous solution
+ *     under the new model.
+ *   Validity: both words integral (-0 is 0) and in range (robot_type 0..3, footprint_type 0..4), and the robot's geometry valid for
+ *     them as above.
+ *   Scope, the setters and the calls refused while records are set: as for the limits records above, word for word
+ *     (mpcb200_set_robot_model: host records, checked, E_INVALID and nothing changes when one is not valid;
+ *     mpcb200_set_robot_model_async: device records, checked per robot by the solve).  Model records combine with limit, geometry
+ *     and weights records: a robot with all four gets all four.
+ */
+#define MPCB200_MODEL_WORDS 2
+#define MPCB200_MOD_ROBOT_TYPE 0      /* MPCB200_ROBOT_*, an integer held as a double */
+#define MPCB200_MOD_FOOTPRINT_TYPE 1  /* MPCB200_FOOTPRINT_*, an integer held as a double */
+int mpcb200_set_robot_model(mpcb200_handle* h, int n, const double* model);
+int mpcb200_set_robot_model_async(mpcb200_handle* h, int n, const double* model);
 
 /*
  * The same solves for a QUEUE of `total` instances (total may exceed max_batch by any factor): the handle's max_batch

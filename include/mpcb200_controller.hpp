@@ -143,7 +143,7 @@ class Controller
         }
         if (!setHorizon(_n_ref)) return false;
         if (_has_limits && !applyRobotLimits()) return false;
-        if (_has_geometry && !applyRobotGeometry()) return false;
+        if (!applyRobotGeometryAndModel()) return false;
         if (_has_weights && !applyRobotWeights()) return false;
         _ocp_seq = 0; _grid_empty = true; _ocp_successful = false;
         return true;
@@ -192,6 +192,37 @@ class Controller
     {
         if (_h) mpcb200_set_robot_geometry(_h, 0, nullptr);
         _has_geometry = false;
+    }
+
+    // Runtime model of this robot (mpcb200_set_robot_model with one record): its robot_type and footprint_type (MPCB200_ROBOT_*,
+    // MPCB200_FOOTPRINT_*) in place of the configuration's -- the reference's robot/type and footprint_model/type without a
+    // reconfigure, e.g. a circular robot that picks up a cart and gets a polygon.  The solves then run the generic kernel key.  The
+    // robot's geometry (setRobotGeometry, else the configuration's values) must be valid for the new types, so a footprint-type
+    // change goes geometry first (a record holding the words of the old and the new footprint, e.g. a radius and a polygon), then
+    // model.  The next step warm-starts from the previous plan under the new model.  The model survives reset(), grid adaptation
+    // and a new configure(); false (and the previous model kept) when the pair is refused (mpcb200.h).
+    bool setRobotModel(int robot_type, int footprint_type)
+    {
+        const double model[MPCB200_MODEL_WORDS] = {(double)robot_type, (double)footprint_type};
+        if (_h && mpcb200_set_robot_model(_h, 1, model) != MPCB200_OK)
+        {
+            std::fprintf(stderr, "Controller::setRobotModel(): %s\n", mpcb200_last_error(_h));
+            return false;
+        }
+        _model[0] = model[0]; _model[1] = model[1];
+        _has_model = true;
+        return true;
+    }
+    // back to the configuration's types; false (and the model kept) when the robot's geometry record is not valid for them
+    bool clearRobotModel()
+    {
+        if (_h && mpcb200_set_robot_model(_h, 0, nullptr) != MPCB200_OK)
+        {
+            std::fprintf(stderr, "Controller::clearRobotModel(): %s\n", mpcb200_last_error(_h));
+            return false;
+        }
+        _has_model = false;
+        return true;
     }
 
     // Runtime objective weights of this robot (mpcb200_set_robot_weights with one record, MPCB200_WGT_* words): Q, R, Qf and the
@@ -382,6 +413,17 @@ class Controller
         std::fprintf(stderr, "Controller: robot geometry: %s\n", mpcb200_last_error(_h));
         return false;
     }
+    // the geometry and model records on a new handle: the geometry first when the handle's own types accept it, else the model
+    // first (checked against the configuration's geometry values)
+    bool applyRobotGeometryAndModel()
+    {
+        if (!_has_model) return !_has_geometry || applyRobotGeometry();
+        const auto model = [&] { return mpcb200_set_robot_model(_h, 1, _model) == MPCB200_OK; };
+        const auto geometry = [&] { return !_has_geometry || mpcb200_set_robot_geometry(_h, 1, _geometry) == MPCB200_OK; };
+        if ((geometry() && model()) || (model() && geometry())) return true;
+        std::fprintf(stderr, "Controller: robot model: %s\n", mpcb200_last_error(_h));
+        return false;
+    }
     bool applyRobotWeights()
     {
         if (mpcb200_set_robot_weights(_h, 1, _weights) == MPCB200_OK) return true;
@@ -415,6 +457,8 @@ class Controller
     bool _has_geometry = false; // setRobotGeometry in effect
     double _weights[MPCB200_WEIGHT_WORDS] = {};
     bool _has_weights = false;  // setRobotWeights in effect
+    double _model[MPCB200_MODEL_WORDS] = {};
+    bool _has_model = false;    // setRobotModel in effect
 };
 
 }  // namespace mpcb200

@@ -48,6 +48,9 @@ GEO_WHEELBASE, GEO_LENGTH_REAR, GEO_LENGTH_FRONT, GEO_FOOTPRINT, GEO_N_POLY, GEO
 # per-robot weights (mpcb200_set_robot_weights): words of a record
 WEIGHT_WORDS = 24
 WGT_Q, WGT_R, WGT_QF, WGT_VP_POSITION, WGT_VP_ORIENTATION = 0, 9, 13, 22, 23
+# per-robot model (mpcb200_set_robot_model): words of a record
+MODEL_WORDS = 2
+MOD_ROBOT_TYPE, MOD_FOOTPRINT_TYPE = 0, 1
 SOLVE_FUSED, SOLVE_PHASED = 0, 1
 NUM_PHASES = 5
 K_H, K_G, K_A, K_B, K_E, K_C, K_HB, K_D = 0, 15, 20, 23, 29, 32, 34, 39
@@ -221,6 +224,7 @@ EXPORTS = [
     "mpcb200_set_robot_limits", "mpcb200_set_robot_limits_async",
     "mpcb200_set_robot_geometry", "mpcb200_set_robot_geometry_async",
     "mpcb200_set_robot_weights", "mpcb200_set_robot_weights_async",
+    "mpcb200_set_robot_model", "mpcb200_set_robot_model_async",
 ]
 
 
@@ -250,6 +254,8 @@ def load_library(path=None):
     lib.mpcb200_set_robot_geometry_async.argtypes = [vp, C.c_int, vp]
     lib.mpcb200_set_robot_weights.argtypes = [vp, C.c_int, dp]
     lib.mpcb200_set_robot_weights_async.argtypes = [vp, C.c_int, vp]
+    lib.mpcb200_set_robot_model.argtypes = [vp, C.c_int, dp]
+    lib.mpcb200_set_robot_model_async.argtypes = [vp, C.c_int, vp]
     lib.mpcb200_solve_stream.argtypes = [vp, C.c_int, dp, dp, dp, C.c_double, C.POINTER(Obstacles), C.POINTER(ViaPoints),
                                          dp, dp, dp, ip, dp, ip, dp]
     lib.mpcb200_reset.argtypes = [vp, ucp, C.c_int]
@@ -521,6 +527,29 @@ class BatchSolver:
             return
         p = _tensor_ptr(t, "weights", torch.float64, self.device, (None, WEIGHT_WORDS))
         self._check(self.lib.mpcb200_set_robot_weights_async(self.h, int(t.shape[0]), p), "mpcb200_set_robot_weights_async")
+
+    def set_robot_model(self, a):
+        """Per-robot model (mpcb200_set_robot_model): a = [n, MODEL_WORDS] (robot_type, footprint_type per robot, integers held as
+        doubles) replaces the handle's two types for robots 0..n-1 of every later solve, which runs the generic kernel key; each
+        robot's geometry (its geometry record, else the configuration's) must be valid for its types.  None clears."""
+        if a is None:
+            self._check(self.lib.mpcb200_set_robot_model(self.h, 0, None), "mpcb200_set_robot_model")
+            return
+        a = np.ascontiguousarray(a, dtype=np.float64)
+        if a.ndim != 2 or a.shape[1] != MODEL_WORDS:
+            raise ValueError(f"model must have shape [n, {MODEL_WORDS}], got {a.shape}")
+        self._check(self.lib.mpcb200_set_robot_model(self.h, a.shape[0], _dp(a)), "mpcb200_set_robot_model")
+
+    def set_robot_model_async(self, t):
+        """set_robot_model() from a torch CUDA tensor float64 [n, MODEL_WORDS] (mpcb200_set_robot_model_async): copied on the
+        handle's stream, which must be torch's current stream; the solve checks each robot's pair of model and geometry (an invalid
+        one makes its robot STATUS_INVALID_INPUT).  None clears."""
+        torch = self._async_prologue()
+        if t is None:
+            self._check(self.lib.mpcb200_set_robot_model_async(self.h, 0, None), "mpcb200_set_robot_model_async")
+            return
+        p = _tensor_ptr(t, "model", torch.float64, self.device, (None, MODEL_WORDS))
+        self._check(self.lib.mpcb200_set_robot_model_async(self.h, int(t.shape[0]), p), "mpcb200_set_robot_model_async")
 
     def upload(self, x0, xf, u_prev=None, u_prev_dt=0.0, obstacles=None, viapoints=None, x_init=None):
         B, x0, xf, u_prev, o, v, xi, keep = self._prep_inputs(x0, xf, u_prev, obstacles, viapoints, x_init)

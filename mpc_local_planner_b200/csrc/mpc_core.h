@@ -153,7 +153,8 @@ HD inline void apply_robot_limits(Cfg& c, const double* r)
 }
 
 // ---- per-robot geometry (mpcb200_set_robot_geometry): a record of MPCB200_GEOMETRY_WORDS doubles ----
-// robot_type and footprint_type stay the handle's; a record supplies the values those two types read and nothing else, so the
+// robot_type and footprint_type stay the handle's (unless model records are set: robot_model_valid); a record supplies the values
+// those two types read and nothing else, so the
 // check and the patch look at exactly those words (the others may hold anything, NaN included).  The blocking setter checks every
 // record with this on the host, the solve kernel checks the record of each robot with it in the instance's prologue.
 HD inline bool geo_finite(double v) { return v >= -1.7976931348623157e308 && v <= 1.7976931348623157e308; }
@@ -221,6 +222,44 @@ HD inline void apply_robot_geometry(Cfg& c, const double* r)
 HD inline bool reads_geometry(const Cfg& c)
 {
     return c.robot_type != MPCB200_ROBOT_UNICYCLE || c.footprint_type != MPCB200_FOOTPRINT_POINT;
+}
+
+// ---- per-robot model (mpcb200_set_robot_model): a record of MPCB200_MODEL_WORDS doubles, robot_type and footprint_type ----
+// A record changes the two types and nothing else: the row set, the objective, the grid and the kernel variant stay the handle's, and
+// the solve runs the MODEL_GENERIC key, which reads both types from the configuration.  A record is valid when both words are
+// integers in range (-0 is 0) and the geometry the robot uses is valid for its types (robot_geometry_valid on the configuration
+// patched with the record's types): its geometry record `geo` when geometry records are set, else the configuration's own values
+// as a record holds them (geometry_record_of).  The blocking setters check every record with this on the host, the solve kernel
+// checks the record of each robot with it in the instance's prologue.
+
+// the record holding a configuration's own geometry values in every word (what apply_robot_geometry writes back unchanged)
+HD inline void geometry_record_of(const Cfg& c, double* r)
+{
+    r[MPCB200_GEO_WHEELBASE] = c.wheelbase;
+    r[MPCB200_GEO_LENGTH_REAR] = c.length_rear;
+    r[MPCB200_GEO_LENGTH_FRONT] = c.length_front;
+    for (int i = 0; i < 4; ++i) r[MPCB200_GEO_FOOTPRINT + i] = c.footprint_params[i];
+    r[MPCB200_GEO_N_POLY] = (double)c.n_poly;
+    for (int i = 0; i < 2 * MPCB200_MAX_POLY; ++i) r[MPCB200_GEO_POLY_XY + i] = c.poly_xy[i];
+}
+HD inline bool model_word_valid(double v, int max) { return v >= 0.0 && v <= (double)max && v == floor(v); }
+// the configuration of a robot: the record's two types, every other field untouched
+HD inline void apply_robot_model(Cfg& c, const double* m)
+{
+    c.robot_type = (int)m[MPCB200_MOD_ROBOT_TYPE];
+    c.footprint_type = (int)m[MPCB200_MOD_FOOTPRINT_TYPE];
+}
+HD inline bool robot_model_valid(const Cfg& c0, const double* m, const double* geo)
+{
+    if (!model_word_valid(m[MPCB200_MOD_ROBOT_TYPE], MPCB200_ROBOT_KIN_BICYCLE) ||
+        !model_word_valid(m[MPCB200_MOD_FOOTPRINT_TYPE], MPCB200_FOOTPRINT_POLYGON))
+        return false;
+    Cfg t = c0;   // (robot_geometry_valid reads the two types of t and nothing else)
+    apply_robot_model(t, m);
+    if (geo) return robot_geometry_valid(t, geo);
+    double r[MPCB200_GEOMETRY_WORDS];
+    geometry_record_of(c0, r);
+    return robot_geometry_valid(t, r);
 }
 
 // ---- per-robot weights (mpcb200_set_robot_weights): a record of MPCB200_WEIGHT_WORDS doubles ----

@@ -27,7 +27,7 @@
 #include <vector>
 
 #include "mpc_device.cuh"
-#ifndef MPCB200_WEIGHTS_UNIT
+#ifndef MPCB200_ENTRY_UNIT
 #include "mpc_costmap.cuh"
 #endif
 #include "mpc_gate.h"
@@ -49,9 +49,10 @@
 // (fold_counters_kernel): cycle words as cycles per CTA of their own launch, the other words as counts
 #define CNT_BYTES (CNT_WORDS * 8 * 2)
 
-// mpcb200_weights.cu compiles this file with MPCB200_WEIGHTS_UNIT defined: the device code the solve kernel is made of and the
-// kernel-variant tables, without the other kernels and the host side, for the per-robot-weights entries it instantiates.
-#ifndef MPCB200_WEIGHTS_UNIT
+// mpcb200_weights.cu and mpcb200_models.cu compile this file with MPCB200_ENTRY_UNIT defined: the device code the solve kernel is
+// made of and the kernel-variant tables, without the other kernels and the host side, for the solve entries each instantiates (the
+// per-robot-weights and the per-robot-model entries).
+#ifndef MPCB200_ENTRY_UNIT
 // ---- kernel: inputs of a batch into the instance blocks (phased path; the fused kernel scatters into shared memory itself) ----
 __global__ void scatter_inputs_kernel(WsLayout L, double* ws, int B, InputPtrs in)
 {
@@ -258,7 +259,7 @@ __device__ __forceinline__ int history_key(const int* prev_iters, const int* pre
     const int k = prev_status[i] == MPCB200_STATUS_MAX_TIME ? max_iter : prev_iters[i];
     return k < 0 ? 0 : (k > 1023 ? 1023 : k);
 }
-#ifndef MPCB200_WEIGHTS_UNIT
+#ifndef MPCB200_ENTRY_UNIT
 __global__ void __launch_bounds__(1024) order_by_history_kernel(const int* __restrict__ prev_iters, const int* __restrict__ prev_status, int max_iter,
                                                                 int B, int* __restrict__ order, int* place, int slots, double rho,
                                                                 int max_heavy, int* queue)
@@ -332,9 +333,11 @@ struct RobotArgs
 // record of each robot (mpcb200_set_robot_geometry, `geo`) is applied to the CTA's configuration after them.
 // WEIGHTS (with ROBOT): the per-robot-weights form -- the limits and geometry records are optional (r.limits, geo may be null; geometry
 // only in the MODEL_GENERIC instantiations), and the weights record of each robot (mpcb200_set_robot_weights, `wgt`) is applied last.
-template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI, bool ROBOT, bool FLEET = false, bool WEIGHTS = false>
+// MODELS (with ROBOT, MODEL_GENERIC only): the per-robot-model form -- the model record of each robot (mpcb200_set_robot_model, `mdl`)
+// is applied first, then the limits, geometry and weights records of the kinds that are set (r.limits, geo, wgt may be null).
+template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI, bool ROBOT, bool FLEET = false, bool WEIGHTS = false, bool MODELS = false>
 __device__ __forceinline__ void solve_fused(const Cfg& c0, const WsLayout& L, const FusedArgs& a, const RobotArgs& r, const double* geo = nullptr,
-                                            const double* wgt = nullptr)
+                                            const double* wgt = nullptr, const double* mdl = nullptr)
 {
     const Cfg& c = ROBOT ? r.cfg[blockIdx.x] : c0;
     extern __shared__ __align__(128) unsigned char dyn_smem[];
@@ -423,7 +426,30 @@ __device__ __forceinline__ void solve_fused(const Cfg& c0, const WsLayout& L, co
             {
                 if (ROBOT && ok)   // the robot's configuration: its record, checked as the blocking setter checks it
                 {
-                    if constexpr (FLEET)
+                    if constexpr (MODELS)
+                    {
+                        // the types first: the geometry (its record, or the configuration's values) is checked for them, and the
+                        // geometry record's patch writes the fields they read.  Each record rewrites every field it touches, per instance.
+                        Cfg& rc = r.cfg[blockIdx.x];
+                        const double* m = mdl + (int64_t)src * MPCB200_MODEL_WORDS;
+                        const double* g = geo ? geo + (int64_t)src * MPCB200_GEOMETRY_WORDS : nullptr;
+                        ok = robot_model_valid(c0, m, g);
+                        if (ok) apply_robot_model(rc, m);
+                        if (ok && r.limits)
+                        {
+                            const double* rec = r.limits + (int64_t)src * MPCB200_LIMIT_WORDS;
+                            ok = robot_limits_valid(c0, rec);
+                            if (ok) apply_robot_limits(rc, rec);
+                        }
+                        if (ok && g) apply_robot_geometry(rc, g);
+                        if (ok && wgt)
+                        {
+                            const double* w = wgt + (int64_t)src * MPCB200_WEIGHT_WORDS;
+                            ok = robot_weights_valid(c0, w);
+                            if (ok) apply_robot_weights(rc, w);
+                        }
+                    }
+                    else if constexpr (FLEET)
                     {
                         // every field a phase reads is rewritten here for each instance: nothing of the CTA's previous robot is left
                         Cfg& rc = r.cfg[blockIdx.x];
@@ -580,8 +606,17 @@ __global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve
 {
     solve_fused<LINES, EXT, WARPS, MODEL, MULTI, true, false, true>(c, L, a, r, geometry, weights);
 }
+// the per-robot-model form (built for MODEL_GENERIC only, which reads both types from the configuration): the same solve, the CTA's
+// configuration patched with its current robot's model record, then its limits, geometry and weights records where those are set
+template <bool LINES, bool EXT, int WARPS, int MODEL, bool MULTI>
+__global__ void __launch_bounds__(WARPS * 32, FusedShape<WARPS>::MIN_CTAS) solve_fused_models_kernel(const __grid_constant__ Cfg c, const __grid_constant__ WsLayout L,
+                                                                                                    const __grid_constant__ FusedArgs a, const __grid_constant__ RobotArgs r,
+                                                                                                    const double* geometry, const double* weights, const double* model)
+{
+    solve_fused<LINES, EXT, WARPS, MODEL, MULTI, true, false, false, true>(c, L, a, r, geometry, weights, model);
+}
 
-#ifndef MPCB200_WEIGHTS_UNIT
+#ifndef MPCB200_ENTRY_UNIT
 // ---- kernel: multistart selection, one warp per robot: the winner among the K candidates (multistart_winner), its state into
 //      slot b (and the resident obstacles' list indices of a long list), its results into output row b ----
 __global__ void multistart_select_kernel(WsLayout L, double* ws, int B, int K, double hysteresis, int long_list, OutputPtrs o, int* winner)
@@ -722,7 +757,13 @@ struct mpcb200_handle
     double* d_geometry = nullptr;    // [max_batch][MPCB200_GEOMETRY_WORDS]
     int robot_weights_n = 0;         // records of per-robot weights in d_weights (0: none; > 0: the solves run solve_fused_weights_kernel)
     double* d_weights = nullptr;     // [max_batch][MPCB200_WEIGHT_WORDS]
-    Cfg* d_robot_cfg = nullptr;      // [robot_cfg_slots] configuration of each CTA of a solve_fused_robot / _fleet / _weights_kernel launch
+    int robot_model_n = 0;           // records of per-robot models in d_model (0: none; > 0: the solves run solve_fused_models_kernel)
+    double* d_model = nullptr;       // [max_batch][MPCB200_MODEL_WORDS]
+    // host copies of the model and geometry records of the blocking setters, which check each kind against the other (empty, and
+    // *_host false, after an async setter: the solve checks those pairs)
+    std::vector<double> h_model, h_geometry;
+    bool model_host = true, geometry_host = true;
+    Cfg* d_robot_cfg = nullptr;      // [robot_cfg_slots] configuration of each CTA of a solve_fused_robot / _fleet / _weights / _models_kernel launch
     int robot_cfg_slots = 0;         // CTAs a solve launch can have: min(max_batch, 32 per SM)
     unsigned long long budget_ns = 0;          // max_cpu_time in ns (0: no budget)
     unsigned long long* d_origin = nullptr;    // start of the current solve launch (%globaltimer), see FusedArgs
@@ -854,7 +895,9 @@ static EntryKernel<E> fused_variant(bool lines, bool ext, bool small, int model,
 // the per-robot-weights entry of a variant (mpcb200_weights.cu): its host function, for cudaFuncSetAttribute, the occupancy query
 // and cudaLaunchKernel
 const void* weights_kernel_variant(bool lines, bool ext, bool small, int model, bool multi);
-#ifndef MPCB200_WEIGHTS_UNIT
+// the per-robot-model entry of a variant (mpcb200_models.cu; MODEL_GENERIC only), for the same uses
+const void* models_kernel_variant(bool lines, bool ext, bool small, bool multi);
+#ifndef MPCB200_ENTRY_UNIT
 using FusedKernel = EntryKernel<FusedEntry>;
 using RobotKernel = EntryKernel<RobotEntry>;
 using FleetKernel = EntryKernel<FleetEntry>;
@@ -986,6 +1029,7 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
     CKC(cudaMalloc(&h->d_limits, B * MPCB200_LIMIT_WORDS * 8)); CKC(cudaMalloc(&h->d_robot_cfg, (size_t)h->robot_cfg_slots * sizeof(Cfg)));
     CKC(cudaMalloc(&h->d_geometry, B * MPCB200_GEOMETRY_WORDS * 8));
     CKC(cudaMalloc(&h->d_weights, B * MPCB200_WEIGHT_WORDS * 8));
+    CKC(cudaMalloc(&h->d_model, B * MPCB200_MODEL_WORDS * 8));
     CKC(cudaMalloc(&h->d_counters, CNT_BYTES)); CKC(cudaMemsetAsync(h->d_counters, 0, CNT_BYTES, h->stream));
     CKC(allow_smem(kkt_warp_kernel<false>)); CKC(allow_smem(kkt_warp_kernel<true>));
     for (const bool lines : {false, true})
@@ -1000,6 +1044,7 @@ extern "C" int mpcb200_create(const mpcb200_config* cfg, int max_batch, int devi
                         CKC(allow_smem(fused_variant<RobotEntry>(lines, ext, small, model, multi)));
                         if (model == MODEL_GENERIC) CKC(allow_smem(fused_variant<FleetEntry>(lines, ext, small, model, multi)));
                         CKC(allow_smem(weights_kernel_variant(lines, ext, small, model, multi)));
+                        if (model == MODEL_GENERIC) CKC(allow_smem(models_kernel_variant(lines, ext, small, multi)));
                     }
         }
     CKC(cudaMallocHost(&h->h_nactive, 8));
@@ -1030,7 +1075,7 @@ extern "C" void mpcb200_destroy(mpcb200_handle* h)
     io_release(h->queue);
     void* ptrs[] = {h->ws, h->d_nactive, h->d_queue, h->d_flush, h->d_counters, h->d_smsync, h->d_prev_iters, h->d_prev_status, h->d_order,
                     h->d_origin, h->d_winner, h->d_resample, h->d_cm, h->d_fz, h->d_limits, h->d_robot_cfg,
-                    h->d_geometry, h->d_weights};
+                    h->d_geometry, h->d_weights, h->d_model};
     for (void* p : ptrs) if (p) cudaFree(p);
     if (h->h_nactive) cudaFreeHost(h->h_nactive);
     for (auto& e : h->ev) cudaEventDestroy(e);
@@ -1084,7 +1129,7 @@ static int group_threads(const mpcb200_handle* h)
 // exist for the kernels without the rarely used obstacle paths only (LINES = false).
 static int kernel_model(const mpcb200_handle* h, const IoBuffers& io)
 {
-    if (io.has_lines || h->force_generic_model) return MODEL_GENERIC;
+    if (io.has_lines || h->force_generic_model || h->robot_model_n > 0) return MODEL_GENERIC;   // (model records: types per robot)
     if (qf_key_matches(h->cfg)) return MODEL_UNI_POINT_QF;
     const bool uni_point = h->cfg.robot_type == MPCB200_ROBOT_UNICYCLE && h->cfg.footprint_type == MPCB200_FOOTPRINT_POINT;
     return uni_point ? MODEL_UNI_POINT : MODEL_GENERIC;
@@ -1219,21 +1264,27 @@ static int launch_fused(mpcb200_handle* h, const IoBuffers& io, int total, int q
     // geometry records: the fleet entry, which applies the limits records too when there are any
     const bool geometry = h->robot_geometry_n > 0 && !queue_mode;
     if (geometry && model != MODEL_GENERIC) return set_err(h, MPCB200_E_UNSUPPORTED, "per-robot geometry needs the generic kernel variant");
-    // weights records: the weights entry, which applies the limits and geometry records too when there are any
-    const bool weights = h->robot_weights_n > 0 && !queue_mode, fleet = geometry && !weights;
-    const FusedKernel kernel = robot || geometry || weights ? nullptr : fused_variant(io.has_lines, ext, small, model, cand_stride > 0);
-    const RobotKernel robot_kernel = robot && !geometry && !weights ? fused_variant<RobotEntry>(io.has_lines, ext, small, model, cand_stride > 0) : nullptr;
+    // model records: the models entry, which applies the limits, geometry and weights records too when there are any (the model
+    // records make the key MODEL_GENERIC, kernel_model); else weights records: the weights entry, which applies the limits and
+    // geometry records too when there are any
+    const bool models = h->robot_model_n > 0 && !queue_mode;
+    const bool weights = h->robot_weights_n > 0 && !queue_mode && !models, fleet = geometry && !weights && !models;
+    const bool per_robot = robot || geometry || weights || models;
+    const FusedKernel kernel = per_robot ? nullptr : fused_variant(io.has_lines, ext, small, model, cand_stride > 0);
+    const RobotKernel robot_kernel = robot && !geometry && !weights && !models ? fused_variant<RobotEntry>(io.has_lines, ext, small, model, cand_stride > 0) : nullptr;
     const FleetKernel fleet_kernel = fleet ? fused_variant<FleetEntry>(io.has_lines, ext, small, model, cand_stride > 0) : nullptr;
     const void* weights_kernel = weights ? weights_kernel_variant(io.has_lines, ext, small, model, cand_stride > 0) : nullptr;
+    const void* models_kernel = models ? models_kernel_variant(io.has_lines, ext, small, cand_stride > 0) : nullptr;
     int per_sm = 0;
-    if (weights) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, weights_kernel, threads, smem));
+    if (models) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, models_kernel, threads, smem));
+    else if (weights) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, weights_kernel, threads, smem));
     else if (fleet) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fleet_kernel, threads, smem));
     else if (robot) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, robot_kernel, threads, smem));
     else CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
     if (per_sm < 1) return set_err(h, MPCB200_E_UNSUPPORTED, "the solve kernel does not fit on an SM with this configuration");
     if (h->max_ctas_per_sm > 0 && per_sm > h->max_ctas_per_sm) per_sm = h->max_ctas_per_sm;
     const int grid = total < per_sm * h->num_sms ? total : per_sm * h->num_sms;
-    if ((robot || geometry || weights) && grid > h->robot_cfg_slots) return set_err(h, MPCB200_E_UNSUPPORTED, "more CTAs than per-robot configuration slots");
+    if (per_robot && grid > h->robot_cfg_slots) return set_err(h, MPCB200_E_UNSUPPORTED, "more CTAs than per-robot configuration slots");
     h->fused_grid = grid;
     CK(cudaMemsetAsync(h->d_queue, 0, 4, h->stream));
     if (!queue_mode && h->order_by_history && h->hist_B == total && total > h->num_sms)
@@ -1255,7 +1306,14 @@ static int launch_fused(mpcb200_handle* h, const IoBuffers& io, int total, int q
     // phase alignment pays when several CTAs share an SM (auto: from three CTAs per SM)
     if (h->sm_phase_sync > 0 || (h->sm_phase_sync < 0 && per_sm >= 3 && grid > h->num_sms)) { a.sm_sync = h->d_smsync; a.sm_words = h->num_sms; }
     if (a.sm_sync || a.place) CK(cudaMemsetAsync(h->d_smsync, 0, (size_t)h->num_sms * SMS_WORD_STRIDE * 8, h->stream));
-    if (weights)
+    if (models)
+    {
+        RobotArgs ra{robot ? h->d_limits : nullptr, h->d_robot_cfg};
+        const double *geo = geometry ? h->d_geometry : nullptr, *wgt = h->robot_weights_n > 0 ? h->d_weights : nullptr, *mdl = h->d_model;
+        void* args[] = {&h->cfg, &h->L, &a, &ra, &geo, &wgt, &mdl};
+        CK(cudaLaunchKernel(models_kernel, dim3(grid), dim3(threads), args, smem, h->stream));
+    }
+    else if (weights)
     {
         RobotArgs ra{robot ? h->d_limits : nullptr, h->d_robot_cfg};
         const double *geo = geometry ? h->d_geometry : nullptr, *wgt = h->d_weights;
@@ -1350,10 +1408,11 @@ static int check_budget_mode(mpcb200_handle* h)
 // persistent kernel (the phased mode has no per-robot form).  Checked before anything is enqueued.
 static int check_robot_limits(mpcb200_handle* h, int robots)
 {
-    if (h->robot_limits_n == 0 && h->robot_geometry_n == 0 && h->robot_weights_n == 0) return 0;
+    if (h->robot_limits_n == 0 && h->robot_geometry_n == 0 && h->robot_weights_n == 0 && h->robot_model_n == 0) return 0;
     if (h->solve_mode == 1)
         return set_err(h, MPCB200_E_UNSUPPORTED, std::string(h->robot_limits_n > 0 ? "per-robot limits need" :
-                                                             h->robot_geometry_n > 0 ? "per-robot geometry needs" : "per-robot weights need") +
+                                                             h->robot_geometry_n > 0 ? "per-robot geometry needs" :
+                                                             h->robot_weights_n > 0 ? "per-robot weights need" : "per-robot models need") +
                                                  " the fused solve kernel (MPCB200_OPT_SOLVE_MODE 0)");
     if (h->robot_limits_n > 0 && robots > h->robot_limits_n)
         return set_err(h, MPCB200_E_INVALID, "per-robot limits: " + std::to_string(robots) + " robots, " + std::to_string(h->robot_limits_n) +
@@ -1364,6 +1423,9 @@ static int check_robot_limits(mpcb200_handle* h, int robots)
     if (h->robot_weights_n > 0 && robots > h->robot_weights_n)
         return set_err(h, MPCB200_E_INVALID, "per-robot weights: " + std::to_string(robots) + " robots, " + std::to_string(h->robot_weights_n) +
                                              " records (mpcb200_set_robot_weights)");
+    if (h->robot_model_n > 0 && robots > h->robot_model_n)
+        return set_err(h, MPCB200_E_INVALID, "per-robot models: " + std::to_string(robots) + " robots, " + std::to_string(h->robot_model_n) +
+                                             " records (mpcb200_set_robot_model)");
     return 0;
 }
 
@@ -1436,6 +1498,7 @@ extern "C" int mpcb200_solve_stream(mpcb200_handle* h, int total, const double* 
     if (h->robot_limits_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "solve_stream with per-robot limits: queue entries are not robots");
     if (h->robot_geometry_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "solve_stream with per-robot geometry: queue entries are not robots");
     if (h->robot_weights_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "solve_stream with per-robot weights: queue entries are not robots");
+    if (h->robot_model_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "solve_stream with per-robot models: queue entries are not robots");
     CK(cudaSetDevice(h->device));
     int rc;
     if ((rc = io_reserve(h, h->queue, (size_t)total, 0))) return rc;
@@ -1600,19 +1663,43 @@ extern "C" int mpcb200_set_robot_limits_async(mpcb200_handle* h, int n, const do
     return MPCB200_OK;
 }
 
+// With model records set, the pairs of model and geometry records the blocking setters would leave (model_n records at `model`,
+// geo_n at `geo`): each robot's geometry (its record, else the configuration's values) valid for its types (its model record,
+// else the handle's).  The first robot whose pair is not valid, or -1.
+static int first_invalid_pair(const Cfg& c, int model_n, const double* model, int geo_n, const double* geo)
+{
+    const int n = model_n > geo_n ? model_n : geo_n;
+    for (int b = 0; b < n; ++b)
+    {
+        const double* g = b < geo_n ? geo + (size_t)b * MPCB200_GEOMETRY_WORDS : nullptr;
+        if (b < model_n ? !robot_model_valid(c, model + (size_t)b * MPCB200_MODEL_WORDS, g) : !robot_geometry_valid(c, g)) return b;
+    }
+    return -1;
+}
+
 // ---- per-robot geometry: records into d_geometry; the solves launch solve_fused_fleet_kernel while robot_geometry_n > 0 ----
 extern "C" int mpcb200_set_robot_geometry(mpcb200_handle* h, int n, const double* geometry)
 {
     if (!h) return MPCB200_E_INVALID;
     if (n < 0 || n > h->max_batch) return set_err(h, MPCB200_E_INVALID, "set_robot_geometry: n must be in [0, max_batch]");
     if (n > 0 && !geometry) return set_err(h, MPCB200_E_INVALID, "set_robot_geometry: geometry is required for n > 0");
-    if (n > 0 && !reads_geometry(h->cfg))
-        return set_err(h, MPCB200_E_INVALID, "set_robot_geometry: a unicycle with a point footprint has no geometry to vary");
-    for (int b = 0; b < n; ++b)
-        if (!robot_geometry_valid(h->cfg, geometry + (size_t)b * MPCB200_GEOMETRY_WORDS))
-            return set_err(h, MPCB200_E_INVALID, "set_robot_geometry: record " + std::to_string(b) + " is not valid (a wheelbase or length_rear "
-                                                 "not finite and > 0, a length_front or radius not finite and >= 0, an offset, line end or vertex "
-                                                 "not finite, or n_poly not an integer in [1, 16])");
+    if (h->robot_model_n == 0)
+    {
+        if (n > 0 && !reads_geometry(h->cfg))
+            return set_err(h, MPCB200_E_INVALID, "set_robot_geometry: a unicycle with a point footprint has no geometry to vary");
+        for (int b = 0; b < n; ++b)
+            if (!robot_geometry_valid(h->cfg, geometry + (size_t)b * MPCB200_GEOMETRY_WORDS))
+                return set_err(h, MPCB200_E_INVALID, "set_robot_geometry: record " + std::to_string(b) + " is not valid (a wheelbase or length_rear "
+                                                     "not finite and > 0, a length_front or radius not finite and >= 0, an offset, line end or vertex "
+                                                     "not finite, or n_poly not an integer in [1, 16])");
+    }
+    else if (h->model_host)   // each record for its robot's types, and the robots without one keep a valid configuration geometry
+    {
+        const int b = first_invalid_pair(h->cfg, h->robot_model_n, h->h_model.data(), n, geometry);
+        if (b >= 0)
+            return set_err(h, MPCB200_E_INVALID, "set_robot_geometry: robot " + std::to_string(b) + " would have a geometry that is not valid "
+                                                 "for the types of its model record (mpcb200_set_robot_model)");
+    }
     CK(cudaSetDevice(h->device));
     if (n > 0)
     {
@@ -1621,6 +1708,8 @@ extern "C" int mpcb200_set_robot_geometry(mpcb200_handle* h, int n, const double
         CK(cudaStreamSynchronize(h->stream));
     }
     h->robot_geometry_n = n;
+    h->h_geometry.assign(geometry, geometry + (size_t)n * MPCB200_GEOMETRY_WORDS);
+    h->geometry_host = true;
     return MPCB200_OK;
 }
 
@@ -1629,7 +1718,7 @@ extern "C" int mpcb200_set_robot_geometry_async(mpcb200_handle* h, int n, const 
     if (!h) return MPCB200_E_INVALID;
     if (n < 0 || n > h->max_batch) return set_err(h, MPCB200_E_INVALID, "set_robot_geometry_async: n must be in [0, max_batch]");
     if (n > 0 && !geometry) return set_err(h, MPCB200_E_INVALID, "set_robot_geometry_async: geometry is required for n > 0");
-    if (n > 0 && !reads_geometry(h->cfg))
+    if (n > 0 && h->robot_model_n == 0 && !reads_geometry(h->cfg))
         return set_err(h, MPCB200_E_INVALID, "set_robot_geometry_async: a unicycle with a point footprint has no geometry to vary");
     CK(cudaSetDevice(h->device));
     if (n > 0)
@@ -1638,6 +1727,8 @@ extern "C" int mpcb200_set_robot_geometry_async(mpcb200_handle* h, int n, const 
         CK(cudaMemcpyAsync(h->d_geometry, geometry, (size_t)n * MPCB200_GEOMETRY_WORDS * 8, cudaMemcpyDeviceToDevice, h->stream));
     }
     h->robot_geometry_n = n;
+    h->h_geometry.clear();
+    h->geometry_host = n == 0;
     return MPCB200_OK;
 }
 
@@ -1678,6 +1769,60 @@ extern "C" int mpcb200_set_robot_weights_async(mpcb200_handle* h, int n, const d
         CK(cudaMemcpyAsync(h->d_weights, weights, (size_t)n * MPCB200_WEIGHT_WORDS * 8, cudaMemcpyDeviceToDevice, h->stream));
     }
     h->robot_weights_n = n;
+    return MPCB200_OK;
+}
+
+// ---- per-robot models: records into d_model; the solves launch solve_fused_models_kernel while robot_model_n > 0 ----
+extern "C" int mpcb200_set_robot_model(mpcb200_handle* h, int n, const double* model)
+{
+    if (!h) return MPCB200_E_INVALID;
+    if (n < 0 || n > h->max_batch) return set_err(h, MPCB200_E_INVALID, "set_robot_model: n must be in [0, max_batch]");
+    if (n > 0 && !model) return set_err(h, MPCB200_E_INVALID, "set_robot_model: model is required for n > 0");
+    for (int b = 0; b < n; ++b)
+    {
+        const double* m = model + (size_t)b * MPCB200_MODEL_WORDS;
+        if (!model_word_valid(m[MPCB200_MOD_ROBOT_TYPE], MPCB200_ROBOT_KIN_BICYCLE) || !model_word_valid(m[MPCB200_MOD_FOOTPRINT_TYPE], MPCB200_FOOTPRINT_POLYGON))
+            return set_err(h, MPCB200_E_INVALID, "set_robot_model: record " + std::to_string(b) + " is not valid (robot_type not an integer in "
+                                                 "[0, 3] or footprint_type not an integer in [0, 4])");
+    }
+    // the geometry records of the blocking setter (or none) against the new types; geometry records of the async setter are the solve's to check
+    if (h->geometry_host)
+    {
+        if (n == 0 && h->robot_geometry_n > 0 && !reads_geometry(h->cfg))
+            return set_err(h, MPCB200_E_INVALID, "set_robot_model: clearing the model records would leave geometry records on a unicycle with a "
+                                                 "point footprint (clear the geometry records first)");
+        const int b = first_invalid_pair(h->cfg, n, model, h->robot_geometry_n, h->h_geometry.data());
+        if (b >= 0)
+            return set_err(h, MPCB200_E_INVALID, "set_robot_model: robot " + std::to_string(b) + " would have a geometry (its geometry record, or "
+                                                 "the configuration's) that is not valid for its types");
+    }
+    CK(cudaSetDevice(h->device));
+    if (n > 0)
+    {
+        CK(cudaMemcpyAsync(h->d_model, model, (size_t)n * MPCB200_MODEL_WORDS * 8, cudaMemcpyHostToDevice, h->stream));
+        h->stats.h2d_bytes += (long long)n * MPCB200_MODEL_WORDS * 8;
+        CK(cudaStreamSynchronize(h->stream));
+    }
+    h->robot_model_n = n;
+    h->h_model.assign(model, model + (size_t)n * MPCB200_MODEL_WORDS);
+    h->model_host = true;
+    return MPCB200_OK;
+}
+
+extern "C" int mpcb200_set_robot_model_async(mpcb200_handle* h, int n, const double* model)
+{
+    if (!h) return MPCB200_E_INVALID;
+    if (n < 0 || n > h->max_batch) return set_err(h, MPCB200_E_INVALID, "set_robot_model_async: n must be in [0, max_batch]");
+    if (n > 0 && !model) return set_err(h, MPCB200_E_INVALID, "set_robot_model_async: model is required for n > 0");
+    CK(cudaSetDevice(h->device));
+    if (n > 0)
+    {
+        if (int rc = check_device_arrays(h, "set_robot_model_async", {model})) return rc;
+        CK(cudaMemcpyAsync(h->d_model, model, (size_t)n * MPCB200_MODEL_WORDS * 8, cudaMemcpyDeviceToDevice, h->stream));
+    }
+    h->robot_model_n = n;
+    h->h_model.clear();
+    h->model_host = n == 0;
     return MPCB200_OK;
 }
 
@@ -1779,6 +1924,7 @@ extern "C" int mpcb200_run_phase(mpcb200_handle* h, int phase, int B)
     if (h->robot_limits_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot limits (mpcb200_set_robot_limits)");
     if (h->robot_geometry_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot geometry (mpcb200_set_robot_geometry)");
     if (h->robot_weights_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot weights (mpcb200_set_robot_weights)");
+    if (h->robot_model_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot models (mpcb200_set_robot_model)");
     CK(cudaSetDevice(h->device));
     if ((rc = launch_phase(h, phase, B, 0, 1, nullptr, true))) return rc;
     CK(cudaStreamSynchronize(h->stream));
@@ -1824,6 +1970,7 @@ extern "C" int mpcb200_time_phase(mpcb200_handle* h, int phase, int B, int reps,
     if (h->robot_limits_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot limits (mpcb200_set_robot_limits)");
     if (h->robot_geometry_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot geometry (mpcb200_set_robot_geometry)");
     if (h->robot_weights_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot weights (mpcb200_set_robot_weights)");
+    if (h->robot_model_n > 0) return set_err(h, MPCB200_E_UNSUPPORTED, "the phase kernels have no per-robot models (mpcb200_set_robot_model)");
     if (reps < 1) reps = 1;
     CK(cudaSetDevice(h->device));
     double total = 0.0;
@@ -2314,4 +2461,4 @@ extern "C" int mpcb200_step_batch_multi(mpcb200_multi* m, int B, const double* x
     if (solve_time_s) { double mx = 0.0; for (double s_ : secs) mx = s_ > mx ? s_ : mx; *solve_time_s = mx; }
     return MPCB200_OK;
 }
-#endif  // MPCB200_WEIGHTS_UNIT
+#endif  // MPCB200_ENTRY_UNIT

@@ -1,7 +1,7 @@
 // mpcb200_weights.cu -- the per-robot-weights entries of the solve kernel (solve_fused_weights_kernel, mpcb200.cu: the full
 // variant table, 28 instantiations) in a translation unit of their own.  The build compiles it beside mpcb200.cu, so the table
 // adds no time to the library's build, and the compile of mpcb200.cu holds the same kernels as before the table existed.
-#define MPCB200_WEIGHTS_UNIT
+#define MPCB200_ENTRY_UNIT
 #include "mpcb200.cu"
 
 struct WeightsEntry
